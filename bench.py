@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — forecast-steps/sec of the GraphLAM hot path on B200 (contract in the task brief).
+"""bench.py — forecast-steps/sec of the GraphLAM hot path on one H100.
 
 Workload (BASELINE.json configs[1]): MEPS-shaped 268x238 grid (xy shape (268, 238), as the reference's create_graph takes it), multiscale
 mesh (6 561 nodes, 57 616 m2m / 100 656 g2m / 255 136 m2g edges), GraphLAM hidden_dim=64,
@@ -7,7 +7,7 @@ mesh (6 561 nodes, 57 616 m2m / 100 656 g2m / 255 136 m2g edges), GraphLAM hidde
 
 One "step" = one autoregressive forecast step (StepPredictor.forward + boundary mix) for a
 batch of B independent forecasts (default 32: every sample shares graph and weights, so the batch is
-a pure extra row dimension; it also pushes the working set far past the 126 MB L2) on each GPU;
+a pure extra row dimension; it also pushes the working set far past the 50 MB L2) on each GPU;
 value = forecast-steps/sec = N*B*K / t.
   * `value`     : inputs resident in HBM, the step replayed from a CUDA graph.
   * `e2e`       : ARForecaster public call path with HOST (pinned) buffers: every step copies that
@@ -43,7 +43,7 @@ import torch  # noqa: E402
 
 D_STATE, D_FORCING, D_STATIC = 17, 18, 4
 # BASELINE.json configs (1-based as listed there).  Config 2 is the one the metric is quoted on (default); 3 and 4 are
-# the H = 128 / 256 workloads (generic tcgen05 path, tc7.cu), 4 as its single-GPU form (B = 1).
+# the H = 128 / 256 workloads (generic wgmma path, tc7.cu), 4 as its single-GPU form (B = 1).
 CONFIGS = {
     2: dict(grid=(268, 238), hierarchical=False, n_levels=None, model="graph_lam", hidden=64, layers=4, batch=32,
             workload="MEPS 268x238 grid, multiscale mesh, GraphLAM hidden_dim=64, 4 processor layers (BASELINE.json configs[1])"),
@@ -64,7 +64,7 @@ def _peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, not a measurement)"
 
 
 def bind_to_gpu_numa(local_rank):
@@ -95,8 +95,8 @@ def _bf16_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         with open(p) as f:
-            return float(json.load(f).get("bf16_tflops_sustained", 1406.5))
-    return 1400.0
+            return float(json.load(f).get("bf16_tflops_sustained", 989.0))
+    return 989.0
 
 
 class ClockSampler:
@@ -268,7 +268,7 @@ def roofline_m2m(model, B, device, iters=20):
 
 def kernel_table(fc, bufs, peak):
     """One EAGER forecast step with the library's per-launch profile on: [{kernel, us, bytes, gbs, frac}] in launch
-    order.  The step's tensors (hundreds of MB at the bench batch) stream through the 126 MB L2 exactly as in the
+    order.  The step's tensors (hundreds of MB at the bench batch) stream through the 50 MB L2 exactly as in the
     replayed step; the launches are the same ones the CUDA graph holds."""
     import ctypes
 
@@ -429,7 +429,7 @@ def measure_train_step(model, device, B=4, iters=5):
         torch.set_float32_matmul_precision(old)
     return {"batch": B, "ms_per_step": ms_ours, "value": B / (ms_ours * 1e-3), "unit": "training samples/s",
             "ref_cuda_ms_per_step": ms_ref, "ref_cuda_value": B / (ms_ref * 1e-3), "speedup": ms_ref / ms_ours,
-            "what": "forward + backward + AdamW step of one forecast step; ours = tcgen05 forward kernels + hand-written "
+            "what": "forward + backward + AdamW step of one forecast step; ours = wgmma forward kernels + hand-written "
                     "backward (backward.py), reference arm = the reference op sequence under torch autograd with TF32 matmuls"}
 
 
@@ -519,6 +519,20 @@ def measure_partition(cfg_id, device, rank, world, steps, warmup, math="auto", b
     return out
 
 
+def dump_outputs(out_dir, new_state, max_nodes=16384):
+    """Write what the timed path returned in its last step: the new state (B, G, d_state), float32.  At the default
+    batch it exceeds 64 MB, so a fixed sample of grid nodes (seeded, sorted; every batch element and variable) is
+    written: new_state.npy (B, min(G, max_nodes), d_state)."""
+    import numpy as np
+
+    G = new_state.shape[1]
+    gen = torch.Generator().manual_seed(0)
+    nodes = torch.arange(G) if G <= max_nodes else torch.randperm(G, generator=gen)[:max_nodes].sort().values
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "new_state.npy"),
+            new_state[:, nodes.to(new_state.device)].float().cpu().numpy())
+
+
 def run_ours(args):
     import torch.distributed as dist
 
@@ -573,11 +587,14 @@ def run_ours(args):
 
         def graphed_steps(t0, n):
             # one AR step = stage this step's forcing / boundary (already in HBM) + replay the captured step; the
-            # state feedback is a rotation of the captured graphs' three state buffers (no copies)
+            # state feedback is a rotation of the captured graphs' three state buffers (no copies).  Returns the buffer
+            # holding the last step's new state.
+            new_state = None
             for i in range(t0, t0 + n):
                 bufs["forcing"].copy_(d_forc[:, i])
                 bufs["boundary"].copy_(d_bnd[:, i])
-                fc.replay_step()
+                new_state = fc.replay_step()
+            return new_state
 
         fc.set_state(d_init[:, 0], d_init[:, 1])
         graphed_steps(0, W)
@@ -585,10 +602,12 @@ def run_ours(args):
         with ClockSampler(local_rank) as clk:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            graphed_steps(W, K)
+            last_state = graphed_steps(W, K)
             e1.record()
             barrier()
             dev_ms = e0.elapsed_time(e1)
+            if args.dump_outputs and rank == 0:
+                dump_outputs(args.dump_outputs, last_state)
             # keep the sampler alive for at least ~0.5 s of load for short runs
             if dev_ms < 500:
                 t_end = time.time() + 0.6
@@ -641,8 +660,8 @@ def run_ours(args):
         tf32_peak = 0.5 * _bf16_peak()
         step_roof = {"algorithmic_bytes": sb, "flops": sf, "hbm_gbs": sb / t_step / 1e9, "hbm_frac": sb / t_step / 1e9 / peak,
                      "tflops": sf / t_step / 1e12, "tensor_frac": sf / t_step / 1e12 / tf32_peak,
-                     "tensor_peak": tf32_peak, "tensor_peak_source": "0.5 x measured dense bf16 (MEASURED_PEAKS.json); a TF32 "
-                     "peak was not measured", "binding": "tensor" if sf / tf32_peak / 1e12 > sb / peak / 1e9 else "hbm"}
+                     "tensor_peak": tf32_peak, "tensor_peak_source": "0.5 x dense bf16 (MEASURED_PEAKS.json if present, else the H100 "
+                     "SXM data sheet's 989 TFLOP/s); a TF32 peak was not measured", "binding": "tensor" if sf / tf32_peak / 1e12 > sb / peak / 1e9 else "hbm"}
         kernels = kernel_table(fc, bufs, peak)
         train = None
         if not args.no_train:
@@ -684,7 +703,7 @@ def run_ours(args):
             "config": {"workload": CFG["workload"],
                        "batch_per_gpu": B, "global_batch": world * B, "math": args.math,
                        "parallelism": f"replicas x{world} (independent forecasts per GPU, no collective)",
-                       "l2": "per-step working set (~0.36 GB x B algorithmic) exceeds the 126 MB L2; "
+                       "l2": "per-step working set (~0.36 GB x B algorithmic) exceeds the 50 MB L2; "
                              "roofline kernel timed with an explicit 256 MB L2 flush between iterations",
                        "cuda_graph": True, "numa_node_rank0": numa_node},
             "e2e": {"value": world * B * K / (e2e_ms * 1e-3), "unit": "forecast-steps/s",
@@ -766,7 +785,14 @@ def main():
                     help="replicas: independent forecasts per GPU (weak scaling, the headline line); partition: ONE batch "
                          "on the node-partitioned graph (strong scaling; --config selects the workload, default 4)")
     ap.add_argument("--cpu-at-scale", action="store_true", help="time the CPU port even for config 4 (minutes)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's new state (a fixed sample of grid nodes) as "
+                         "DIR/new_state.npy (float32); inputs and weights are seeded, so runs with the same arguments "
+                         "are comparable output for output")
     args = ap.parse_args()
+    if args.dump_outputs and (args.parallelism == "partition" or args.impl == "reference"):
+        ap.error("--dump-outputs writes the replicated device-resident step's outputs: not available with "
+                 "--parallelism partition or --impl reference")
     global CFG, METRIC
     CFG = CONFIGS[args.config]
     METRIC = ("forecast-steps/sec (268x238 grid, hidden=64)" if args.config == 2 else

@@ -1,5 +1,5 @@
 /*
- * nlam_b200.h — C ABI of libnlam_b200.so: B200 (sm_100a) kernels for the Neural-LAM
+ * nlam_b200.h — C ABI of libnlam_b200.so: H100 (sm_90a) kernels for the Neural-LAM
  * InteractionNet message-passing hot path.
  *
  * This is the drop-in boundary.  The reference has no native code at all: the path is
@@ -54,7 +54,7 @@ extern "C" {
 /* flags for nlam_inet_fwd / nlam_rowmlp_fwd */
 #define NLAM_AGGR_MEAN 0x1        /* mean instead of sum aggregation */
 #define NLAM_PROPAGATION 0x2      /* PropagationNet: msg = x_j + mlp(..), node residual = aggr */
-#define NLAM_MATH_TF32 0x10       /* tcgen05 TF32 tensor-core kernels (fp32 accumulate) */
+#define NLAM_MATH_TF32 0x10       /* wgmma TF32 tensor-core kernels (fp32 accumulate) */
 #define NLAM_MATH_FP32 0x20       /* exact fp32 FFMA kernels */
 #define NLAM_HINT_ONE_HIDDEN 0x100 /* promise to nlam_inet_workspace_bytes: both MLPs are Linear-SiLU-Linear-LayerNorm */
 #define NLAM_EDGE_ONLY 0x200      /* nlam_inet_fwd: stop after the aggregation (aggr_out required; rec_out unused): the node
@@ -120,7 +120,7 @@ int32_t nlam_graph_max_in_degree(const NlamGraph* g);
 int32_t nlam_graph_is_sorted(const NlamGraph* g);   /* 1 if the given order already is CSR order */
 /* d if every receiver has exactly d incoming edges (mesh->grid: 4 nearest mesh nodes, reference
  * create_graph.py:779-792; mesh-down: one parent), else 0; such edge sets with update_edges=False take the
- * receiver-tiled kernels.  ell_window: 1 if additionally every 128-receiver tile reads <= 128 distinct senders. */
+ * receiver-tiled kernels.  ell_window: 1 if additionally d <= 8 (the uniform-degree edge path applies). */
 int32_t nlam_graph_uniform_degree(const NlamGraph* g);
 int32_t nlam_graph_ell_window(const NlamGraph* g);
 /* device pointers (int32): receiver CSR, sender CSR (for gather backward), permutations */
@@ -149,7 +149,7 @@ int nlam_inet_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* ag
 
 /* Stack of InteractionNet layers over ONE node set (send == rec: the mesh processor, reference graph_lam.py:117-126).  With
  * next_edge_mlp + proj_out the node update of this call also computes the node projections of the NEXT layer's edge MLP,
- * P_s = W1s'·x', P_r = W1r'·x' + b1' (proj_out: (2, B, n_rec, 64)), in the same kernel (csrc/tc10.cu); with proj_in the edge stage
+ * P_s = W1s'·x', P_r = W1r'·x' + b1' (proj_out: (2, B, n_rec, 64)), in the same kernel (csrc/fused.cu); with proj_in the edge stage
  * of this call takes its projections from the previous call instead of launching its own projection pass.  Both NULL: exactly
  * nlam_inet_fwd.  nlam_inet_chain_supported says whether a call shape can be a consumer (next_edge_mlp NULL) and a producer. */
 int nlam_inet_chain_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp, const NlamMlp* next_edge_mlp,
@@ -160,7 +160,7 @@ int nlam_inet_fwd_chain(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamM
                         float* proj_out, int B, int flags, void* workspace, size_t ws_bytes, void* stream);
 
 /* 1 if nlam_inet_fwd with these arguments may be called with edge_out == edge (tensor-core path with node projections on a
- * general CSR edge set, dense batches: the update is a TMA reduce-add of the message tiles, csrc/tc8.cu), else 0. */
+ * general CSR edge set, dense batches: each tile reads its edge rows and writes e + m back, csrc/fused.cu), else 0. */
 int nlam_inet_inplace_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bstride,
                                 const float* rec, int64_t rec_bstride, const float* edge, int64_t edge_bstride, int B,
                                 int flags);
@@ -171,7 +171,7 @@ int nlam_rowmlp_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const
                     const NlamRowSrc* res2, float* out, float* out2, int64_t n_rows, int B,
                     int flags, void* stream);
 
-/* Tail of the grid side of a forecast step in one launch (csrc/tc9.cu): the node update of the mesh->grid InteractionNet
+/* Tail of the grid side of a forecast step in one launch (csrc/fused.cu): the node update of the mesh->grid InteractionNet
  *   grid' = rec + node_mlp([rec | aggr])              (reference gnn_layers.py:148-151)
  * chained with output_map and the step epilogue of nlam_rowmlp_step_fwd; grid' never leaves the SM.  rec (B, n_rows, 64)
  * with batch stride rec_bstride, aggr (B, n_rows, 64) dense (nlam_inet_fwd with NLAM_EDGE_ONLY).  NLAM_E_UNSUPPORTED for
@@ -203,7 +203,7 @@ int nlam_halo_push(const float* own, int64_t own_bs, int64_t n_own, float* ext_l
                    float* const* peer_ext, const int32_t* send_rows, const int32_t* send_ptr,
                    const int32_t* peer_dst_off, int64_t n_send_total, int world, int B, int H, void* stream);
 
-/* ---- Backward building blocks (bwd.cu) and the generic tcgen05 Linear (tc7.cu) -------------------------------
+/* ---- Backward building blocks (bwd.cu) and the generic wgmma Linear (tc7.cu) -------------------------------
  * The backward of the path (reference: autograd through gnn_layers.py:110-157 / utils/networks.py:27-40) is composed
  * from these launches by the host side (neural_lam_b200/backward.py): dX = dY · W and dW = dYᵀ · X run on nlam_linear
  * (dW as split-K partial products over zero-padded transposes, reduced in a fixed order by nlam_reduce_partials). */

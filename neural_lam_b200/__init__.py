@@ -1,4 +1,4 @@
-"""neural_lam_b200 — B200 (sm_100a) kernels for Neural-LAM's InteractionNet message-passing
+"""neural_lam_b200 — H100 (sm_90a) kernels for Neural-LAM's InteractionNet message-passing
 hot path behind the reference's Python API (``neural_lam.gnn_layers`` /
 ``neural_lam.models`` GraphLAM / HiLAM).  See DESIGN.md and INTEGRATION.md."""
 from . import _lib, ops  # noqa: F401

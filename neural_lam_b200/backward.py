@@ -3,7 +3,7 @@ InteractionNet / PropagationNet (reference gnn_layers.py:110-157, :231-249; exer
 tests/test_gnn_layers.py section F and by training, models/module.py:303) composed from libnlam_b200 launches only —
 no ATen / cuBLAS math:
 
-  * dense products on the generic tcgen05 Linear kernel (``nlam_linear``, csrc/tc7.cu): ``dX = dY · W`` is a Linear with
+  * dense products on the generic wgmma Linear kernel (``nlam_linear``, csrc/tc7.cu): ``dX = dY · W`` is a Linear with
     the transposed weight, ``dW = dYᵀ · X`` a split-K product over zero-padded transposes of dY and X whose partial
     products are reduced in a fixed order;
   * SiLU / LayerNorm forward + backward, bias column sums, transposes, the gather-add of the message gradient and the
@@ -38,7 +38,7 @@ def _dense3(x):
 
 def linear(x0, w, n_out, *, w_off=0, ldw=None, w_cols=0, w_bs=0, x1=None, bias=None, act=False, ln=None, add=(), post=None,
            res=None, out2=False, x0_pitch=0, k0=None, shape=None, x0_bs=None):
-    """``epi([x0 | x1] · W[:, cols]ᵀ + bias + gathered addends)`` on the generic tcgen05 Linear kernel.
+    """``epi([x0 | x1] · W[:, cols]ᵀ + bias + gathered addends)`` on the generic wgmma Linear kernel.
     x0 / x1: dense (B, n, k) tensors (or, with ``shape=(B, n)``, ``k0`` and ``x0_pitch`` / ``x0_bs``: a raw strided
     view); ``w``: parameter / buffer holding the weight, ``w_off`` its column offset, ``ldw`` its row pitch;
     ``add`` / ``post``: (tensor (B|1, rows, n_out), int32 index pointer, batch stride) gathered addends before / after the

@@ -1,4 +1,4 @@
-// C-ABI entry points that dispatch between the tcgen05 (TF32) kernels and the exact fp32
+// C-ABI entry points that dispatch between the wgmma (TF32) kernels and the exact fp32
 // kernels.  See include/nlam_b200.h for the contract and the reference interfaces replaced.
 #include "common.cuh"
 
@@ -16,7 +16,7 @@ extern "C" int nlam_rowmlp_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n
   if (want_tf32(flags) && tc_rowmlp_supported(mlp, srcs, n_src, res, res2, n_rows))
     return tc_rowmlp(mlp, srcs, n_src, res, out, n_rows, B, st);
   if (want_tf32(flags) && !out2 && tc_mlp2_supported(mlp, srcs, n_src, res, res2)) {
-    // H = 128 / 256: two launches of the generic tcgen05 Linear kernel; the hidden activations live in a
+    // H = 128 / 256: two launches of the generic wgmma Linear kernel; the hidden activations live in a
     // stream-ordered scratch allocation (legal inside a stream capture)
     float* ws = nullptr;
     NLAM_CUDA_OK(cudaMallocAsync((void**)&ws, (size_t)n_rows * B * mlp->out_dim[0] * sizeof(float), st));
@@ -33,7 +33,7 @@ extern "C" int nlam_rowmlp_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n
     return rc;
   }
   NLAM_REQUIRE(!(flags & NLAM_MATH_TF32), NLAM_E_UNSUPPORTED,
-               "nlam_rowmlp_fwd: shape not supported by the tcgen05 kernels (in=%d)", mlp->in_dim);
+               "nlam_rowmlp_fwd: shape not supported by the tensor-core kernels (in=%d)", mlp->in_dim);
   return rowmlp_simt(mlp, srcs, n_src, res, res2, out, out2, n_rows, B, st);
 }
 
@@ -90,7 +90,7 @@ extern "C" size_t nlam_inet_workspace_bytes(const NlamGraph* g, int B, int H, in
   return rup256((size_t)B * g->n_rec * H * sizeof(float)) + need;
 }
 
-// the call shapes that take tc_edge_rmw (tc8.cu) when edge_out aliases edge
+// the call shapes that take tc_edge_rmw (fused.cu) when edge_out aliases edge
 static bool inplace_path(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
                          int64_t rec_bs, const float* edge, int64_t edge_bs, int B, int flags) {
   const int H = edge_mlp->out_dim[edge_mlp->n_linear - 1];
@@ -109,7 +109,7 @@ extern "C" int nlam_inet_inplace_supported(const NlamGraph* g, const NlamMlp* ed
 }
 
 // chain of layers over ONE node set (the mesh processor): can this call consume node projections computed by the previous
-// layer's node kernel and, with next_mlp, produce those of the next layer (tc10.cu)?
+// layer's node kernel and, with next_mlp, produce those of the next layer (fused.cu)?
 static bool chain_path(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp, const NlamMlp* next_mlp,
                        const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, int B, int flags) {
   if (!(want_tf32(flags) && tc_edge_supported(g, edge_mlp, flags)) || (flags & (NLAM_PROPAGATION | NLAM_EDGE_ONLY))) return false;
@@ -189,7 +189,7 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
   const int64_t aggr_bs = (int64_t)g->n_rec * H;
 
   NLAM_REQUIRE(use_tc || use_gen || !(flags & NLAM_MATH_TF32), NLAM_E_UNSUPPORTED,
-               "nlam_inet_fwd: shape (H=%d, max in-degree %d, hidden_layers=%d) not supported by the tcgen05 kernels",
+               "nlam_inet_fwd: shape (H=%d, max in-degree %d, hidden_layers=%d) not supported by the tensor-core kernels",
                H, g->max_in_degree, edge_mlp->n_linear - 1);
   NLAM_REQUIRE(!(use_gen && edge_only), NLAM_E_UNSUPPORTED, "nlam_inet_fwd: NLAM_EDGE_ONLY is not available on the generic path");
   if (use_gen)
@@ -201,11 +201,11 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
     const int64_t send_rows = (B > 1 && send_bs > 0) ? send_bs / H : g->n_send;
     int rc;
     if (tc_ell_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge_out != nullptr)) {
-      // uniform in-degree: receiver-tiled ELL kernel, aggregation in registers (tc3.cu)
+      // uniform in-degree edge sets (fused.cu)
       rc = tc_ell_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, aggr, B, flags, st, scratch);
     } else if (tc_edge2_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, B, send_rows)) {
-      // split first Linear: node projections + K=64 edge kernel with sender windows (tc5.cu)
-      // (tc8.cu when the edge tensor is updated in place or not written at all)
+      // split first Linear: node projections + K=64 edge kernel (fused.cu)
+      // (tc_edge_rmw when the edge tensor is updated in place or not written at all)
       // (projections computed by the previous layer's node kernel: proj_in holds [P_s | P_r] in the scratch layout)
       float* pws = proj_in ? const_cast<float*>(proj_in) : scratch;
       if (tc_edge_rmw_supported(g, edge, edge_bs, edge_out, B))
@@ -214,7 +214,7 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
         rc = tc_edge3(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st, pws, proj_in != nullptr);
     } else if (tc_edge_bcast_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, edge_out != nullptr)) {
       // batch-broadcast edge features and receivers, large sender set, no edge update (grid -> mesh): tile-major
-      // kernel with the edge term resident in TMEM and raw sender rows gathered (tc6.cu)
+      // K = 192 kernel on raw gathered sender rows (fused.cu)
       rc = tc_edge_bcast(g, edge_mlp, send, send_bs, rec, rec_bs, edge, aggr, B, flags, st, scratch);
     } else {
       rc = tc_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st, send_rows);
@@ -235,7 +235,7 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
   // node update: rec' = base + aggr_mlp(cat(rec, aggr)); base = rec (InteractionNet) or aggr (PropagationNet)
   NlamRowSrc nsrcs[2] = {{rec, nullptr, rec_bs, H, 0}, {aggr, nullptr, aggr_bs, H, 0}};
   NlamRowSrc nres = prop ? nsrcs[1] : nsrcs[0];
-  if (next_mlp)  // node update + the next layer's node projections (tc10.cu)
+  if (next_mlp)  // node update + the next layer's node projections (fused.cu)
     return tc_node_proj(aggr_mlp, next_mlp, rec, rec_bs, aggr, g->n_rec, B, rec_out, proj_out, st);
   if (use_tc && tc_rowmlp_supported(aggr_mlp, nsrcs, 2, &nres, nullptr, g->n_rec))
     return tc_rowmlp(aggr_mlp, nsrcs, 2, &nres, rec_out, g->n_rec, B, st);

@@ -3,7 +3,7 @@
 //   dX = dY · W          (Linear with the transposed weight)
 //   dW = dYᵀ · X         (reduction over the rows: split-K partial products on the tensor cores + a deterministic
 //                         reduction of the partials)
-// run on the generic tcgen05 Linear kernel (tc7.cu); this file holds the elementwise / reduction / layout kernels
+// run on the generic wgmma Linear kernel (tc7.cu); this file holds the elementwise / reduction / layout kernels
 // around them: SiLU forward / backward, LayerNorm forward / backward (with the dγ / dβ column reductions), column
 // sums (bias gradients), zero-padded transposes (the K-major operands of the dW products), the reduction of partial
 // products, and the gather-add that assembles the message gradient g_m[e] = g_e'[e] + g_aggr[dst(e)] / deg.
@@ -12,7 +12,7 @@
 
 namespace nlam {
 
-static int grid_1d(long long total, int block, int cap = 148 * 8) {
+static int grid_1d(long long total, int block, int cap = 132 * 8) {
   long long g = (total + block - 1) / block;
   return (int)std::max<long long>(1, std::min<long long>(g, cap));
 }
@@ -278,7 +278,7 @@ extern "C" int nlam_layernorm_fwd(const float* y, const float* gamma, const floa
   return NLAM_OK;
 }
 
-extern "C" size_t nlam_bwd_scratch_floats(int C) { return (size_t)(148 * 8 * 8 + 2) * 2 * (size_t)C; }
+extern "C" size_t nlam_bwd_scratch_floats(int C) { return (size_t)(132 * 8 * 8 + 2) * 2 * (size_t)C; }
 
 extern "C" int nlam_layernorm_bwd(const float* g, const float* y, const float* gamma, float eps, float* gy, float* dgamma,
                                   float* dbeta, int64_t rows, int H, float* scratch, void* stream) {
@@ -307,7 +307,7 @@ extern "C" int nlam_layernorm_bwd(const float* g, const float* y, const float* g
 extern "C" int nlam_colsum(const float* g, int64_t rows, int C, float* out, float* scratch, void* stream) {
   NLAM_REQUIRE(g && out && scratch && C >= 1 && C <= 1024, NLAM_E_INVALID, "nlam_colsum: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  const int grid = grid_1d(std::max<int64_t>(rows, 1) * 32, 256, 148 * 4);
+  const int grid = grid_1d(std::max<int64_t>(rows, 1) * 32, 256, 132 * 4);
   const int n_warps = grid * 8;
   {
     ProfScope ps("colsum_kernel", st, 4.0 * rows * C);
@@ -339,7 +339,7 @@ extern "C" int nlam_transpose_pad(const float* x, int64_t rows, int C, int64_t x
   const long long tiles = ((rows_pad + 31) / 32) * ((C + 31) / 32);
   {
     ProfScope ps("transpose_pad_kernel", st, 4.0 * C * (rows + rows_pad));
-    transpose_pad_kernel<<<(int)std::min<long long>(tiles, 148 * 16), 256, 0, st>>>(x, rows, C, x_pitch, xt, rows_pad);
+    transpose_pad_kernel<<<(int)std::min<long long>(tiles, 132 * 16), 256, 0, st>>>(x, rows, C, x_pitch, xt, rows_pad);
   }
   count_launch();
   NLAM_CUDA_OK(cudaGetLastError());
@@ -361,7 +361,7 @@ extern "C" int nlam_add_gather(const float* a, const float* v, const int32_t* id
   return NLAM_OK;
 }
 
-// Generic tcgen05 Linear through the C ABI (LinearCall fields flattened; see common.cuh / tc7.cu)
+// Generic wgmma Linear through the C ABI (LinearCall fields flattened; see common.cuh / tc7.cu)
 extern "C" int nlam_linear(const float* x0, int64_t x0_bs, int k0, int64_t x0_pitch, const float* x1, int64_t x1_bs, int k1,
                            const float* w, int ldw, int w_cols, int64_t w_bs, const float* bias, int n_out, int act,
                            const float* gamma, const float* beta, float eps, const float* add0, const int32_t* add0_idx,
@@ -473,7 +473,7 @@ static void transpose(Ctx& c, const float* x, int64_t rows, int64_t mod_rows, in
   const long long tiles = ((rows_pad + 31) / 32) * ((C + 31) / 32);
   {
     ProfScope ps("transpose_pad_kernel", c.st, 4.0 * C * (rows + rows_pad));
-    transpose_mod_kernel<<<(int)std::min<long long>(tiles, 148 * 16), 256, 0, c.st>>>(x, rows, mod_rows, C, pitch, xt, rows_pad);
+    transpose_mod_kernel<<<(int)std::min<long long>(tiles, 132 * 16), 256, 0, c.st>>>(x, rows, mod_rows, C, pitch, xt, rows_pad);
   }
   count_launch();
   if (cudaGetLastError() != cudaSuccess) c.rc = NLAM_E_CUDA;

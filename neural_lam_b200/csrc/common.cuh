@@ -1,4 +1,4 @@
-// Shared declarations for libnlam_b200.so (sm_100a only).
+// Shared declarations for libnlam_b200.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,7 +47,7 @@ struct ProfScope {
   ~ProfScope() { prof_end(st); }
 };
 
-constexpr int kTileEdges = 128;  // rows of one tensor-core edge tile (UMMA M)
+constexpr int kTileEdges = 128;  // rows of one tensor-core edge tile
 
 struct StepEpilogue {  // fused forecast-step epilogue of a narrow-output row MLP (see TcParams::ep_*)
   const float* prev;
@@ -56,23 +56,11 @@ struct StepEpilogue {  // fused forecast-step epilogue of a narrow-output row ML
   const float* std;
   const float* mean;
 };
-// tc2.cu: split-first-Linear edge kernel (v2) + node projection kernel
+// fused.cu: split-first-Linear edge kernel (v2) + node projection kernel
 bool tc_edge2_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
                         const float* rec, int64_t rec_bs, int B, int64_t send_rows);
 size_t tc_edge2_workspace_floats(const NlamGraph* g, int B, int64_t send_rows_max);
-// tc2.cu: out = x · wsliceᵀ (+ bias) for 64-wide rows; wslice = 64 columns of a row-major weight with row pitch ldw
-struct RowLinProblem {
-  const float* x;
-  int64_t x_bs;
-  int64_t n_rows;
-  int B_eff;
-  const float* wslice;
-  int ldw;
-  const float* bias;
-  float* out;
-};
-int rowlinear_multi(const RowLinProblem* pr, int n_prob, cudaStream_t st);
-// tc7.cu: generic tcgen05 Linear (any K multiple of 32, N <= 256) and the layer paths built from it
+// tc7.cu: generic wgmma Linear (any K multiple of 32, N <= 256) and the layer paths built from it
 struct LinearCall {
   const float* x0;      // (B|1, n_rows, k0) rows; row pitch x0_pitch (0: dense = k0)
   int64_t x0_bs;
@@ -118,38 +106,31 @@ size_t tc_inet_gen_workspace_floats(const NlamGraph* g, int B, int H);
 int tc_inet_gen(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp, const float* send, int64_t send_bs,
                 const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, float* rec_out, float* edge_out,
                 float* aggr, int B, int flags, float* ws, cudaStream_t st);
-// tc6.cu: batch-broadcast edge features, no edge update, raw sender rows gathered (grid -> mesh)
+// fused.cu: batch-broadcast edge features and receivers, no edge update (grid -> mesh)
 bool tc_edge_bcast_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
                              const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B, bool has_edge_out);
-size_t tc_edge_bcast_workspace_floats(const NlamGraph* g, int B, int64_t rec_bs);
 int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
                   int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws);
-// tc5.cu
+// fused.cu: split form, out-of-place edge output
 int tc_edge3(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
              int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,
              cudaStream_t stream, float* ws, bool have_proj = false);
-// tc8.cu: same math, edge tensor updated in place (TMA reduce-add) or not written at all
+// fused.cu: same math, edge tensor updated in place or not written at all
 bool tc_edge_rmw_supported(const NlamGraph* g, const float* edge, int64_t edge_bs, const float* edge_out, int B);
 int tc_edge_rmw(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
                 int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,
                 cudaStream_t stream, float* ws, bool have_proj = false);
-// tc9.cu: node update of the mesh->grid layer + output_map + step epilogue in one kernel
+// fused.cu: node update of the mesh->grid layer + output_map + step epilogue in one kernel
 bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                            int64_t n_rows, int B, const float* out, const StepEpilogue* ep);
 int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                 int64_t n_rows, int B, float* out, const StepEpilogue* ep, cudaStream_t st);
-// tc10.cu: node update + the next layer's node projections in one kernel (stacks of layers over one node set)
+// fused.cu: node update + the next layer's node projections in one kernel (stacks of layers over one node set)
 bool tc_node_proj_supported(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs,
                             const float* aggr, int64_t n_rows, const float* out, const float* proj_out);
 int tc_node_proj(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                  int64_t n_rows, int B, float* out, float* proj_out, cudaStream_t st);
-// tc4.cu
-bool tc_rowmlp64_supported(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res, int64_t n_rows);
-bool tc_rowmlp_narrow_out_supported(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, int64_t n_rows, const float* out,
-                                    const StepEpilogue* ep);
-int tc_rowmlp64(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res, float* out, int64_t n_rows,
-                int B, cudaStream_t stream, const StepEpilogue* ep = nullptr);
-// tc3.cu
+// fused.cu: uniform in-degree edge sets
 bool tc_ell_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
                       const float* rec, int64_t rec_bs, bool has_edge_out);
 int tc_ell_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
@@ -183,22 +164,7 @@ struct NlamGraph {
   // [rowptr[tile_rec[t]], rowptr[tile_rec[t+1]]).  n_tiles == 0 if some in-degree > 128.
   int32_t n_tiles = 0;
   int32_t* tile_rec = nullptr;  // n_tiles+1
-  int32_t* tile_e0 = nullptr;   // n_tiles+1: first CSR edge of each tile
-  int32_t* tile_meta = nullptr; // 4*n_tiles: {first edge, #edges, first receiver, #receivers}
-  // uniform in-degree (ELL) sender windows: receiver tile t (128 receivers) reads ell_nu[t] <= 128 distinct
-  // senders ell_u[128*t ..] (ascending, padded to a multiple of 4); CSR edge k reads window row ell_loc[k].
-  // ell_window == 0 if some tile reads more than 128 distinct senders (or the degree is not uniform).
-  int32_t ell_window = 0;
-  int32_t ell_nt = 0;           // number of ELL receiver tiles
-  int32_t* ell_r0 = nullptr;    // ell_nt + 1: first receiver of every ELL tile (tile t = receivers [ell_r0[t], ell_r0[t+1]), <= 128)
-  int32_t* ell_u = nullptr;
-  int32_t* ell_nu = nullptr;
-  uint8_t* ell_loc = nullptr;
-  // sender windows of the CSR tiles (tc2.cu): the 128-edge window of tile t reads win_nu[t] <= 128 distinct
-  // senders win_u[128*t ..] (ascending, padded to a multiple of 4); its row i reads window row win_loc[128*t + i]
-  int32_t* win_u = nullptr;
-  int32_t* win_nu = nullptr;
-  uint8_t* win_loc = nullptr;
+  int32_t ell_window = 0;       // 1: uniform in-degree <= 8 (the uniform-degree edge path)
   std::vector<int32_t> h_tile_rec, h_rowptr;
 };
 
@@ -216,7 +182,7 @@ inline double edge_algorithmic_bytes(const NlamGraph* g, int B, int64_t send_bs,
 int rowmlp_simt(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res,
                 const NlamRowSrc* res2, float* out, float* out2, int64_t n_rows, int B,
                 cudaStream_t stream);
-// tc.cu
+// fused.cu
 bool tc_rowmlp_supported(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res,
                          const NlamRowSrc* res2, int64_t n_rows);
 int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res,

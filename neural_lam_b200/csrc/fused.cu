@@ -1,0 +1,797 @@
+// Fused H = 64 kernels for sm_90a (wgmma TF32, fp32 accumulate): one CTA works on tiles of 128 rows (node rows, or the CSR
+// edges of whole receivers), two warp groups own 64 rows each.  Per tile:
+//
+//   A  = [src_0 | src_1 | ...] rows (gathered through row indices, zero-padded to a multiple of 32 columns) -> shared memory
+//   h  = SiLU(A · W1ᵀ + b1 [+ P_s[src] + P_r[dst]])        wgmma, accumulators in registers, h back to shared memory
+//   y  = LN(h · W2ᵀ + b2) [+ residual]                     wgmma
+//
+// then one of: the row output (optionally the forecast-step epilogue), the edge output e' = e + y together with the
+// deterministic per-receiver sum of y over the tile's edges (every receiver lies in one tile), or two more 64-wide GEMMs on
+// y (the next layer's node projections; or output_map and the step epilogue).  All weights of a launch stay in shared
+// memory for the whole persistent CTA; operands are written in the 128-byte swizzle wgmma reads, and every generic-proxy
+// write of an operand is followed by fence.proxy.async before the warp group's MMAs read it.
+//
+// Launch names (nlam_profile_*): tc_rowmlp_kernel (row MLPs, node updates, output_map + step epilogue),
+// tc_rowlinear_kernel (node projections P_s = x_s·W1sᵀ, P_r = x_r·W1rᵀ + b1 of the split first edge Linear, both node
+// sets in one grid), tc_edge_kernel (K = 192 edge MLP on raw gathered rows), tc_edge3_kernel (split form, out-of-place
+// edge output), tc_edge_rmw_kernel (split form, edge tensor updated in place or not written), tc_ell_window_kernel
+// (uniform in-degree edge sets), tc_edge_bcast_kernel (batch-broadcast edge features and receivers, split form),
+// tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
+// epilogue).
+#include "tc_ptx.cuh"
+#include "wgmma_tf32.cuh"
+
+namespace nlam {
+
+namespace fz {
+constexpr int THREADS = 256;
+constexpr uint32_t CH_A = 128 * 128;  // one 32-column chunk of a 128-row operand
+constexpr uint32_t CH_W = 64 * 128;   // one 32-column chunk of a 64-row weight
+constexpr uint32_t OFF_A = 0;
+// Shared memory, sized per launch so that the K = 64 launches fit two CTAs per SM:
+//   A (max(kc1, 2) chunks) | W1 (kc1 chunks) | W2 (2) | W3, W4 (2 + 2; for the edge modes the 128 x 64 fp32 message buffer)
+//   | b1 | b2 | gamma | beta | b3 | b4 | b1 of problem 1 (64 floats each)
+struct Layout {
+  uint32_t w1, w2, w3, w4, prm, bytes;
+};
+__host__ __device__ inline Layout layout(int kc1, int mode, int post) {
+  Layout l;
+  l.w1 = (uint32_t)(kc1 > 2 ? kc1 : 2) * CH_A;
+  l.w2 = l.w1 + (uint32_t)kc1 * CH_W;
+  l.w3 = l.w2 + 2 * CH_W;
+  l.w4 = l.w3 + 2 * CH_W;
+  const uint32_t tail = (post != 0 || mode == 1) ? 4 * CH_W : (mode == 2 ? 2 * CH_W : 0);
+  l.prm = l.w3 + tail;
+  l.bytes = l.prm + 7 * 64 * 4 + 1024;  // + alignment slack
+  return l;
+}
+enum Mode { ROWS = 0, EDGE = 1, ROWLIN = 2 };
+enum Post { POST_NONE = 0, POST_PROJ = 1, POST_OUTMLP = 2 };
+}  // namespace fz
+
+struct FzSrc {
+  const float* ptr;
+  const int32_t* idx;  // row r reads row idx[r] (NULL: row r)
+  long long bs;        // batch stride in elements (0: broadcast)
+  int dim;
+};
+struct FzW {           // rows x cols slice of a row-major matrix with row pitch ld
+  const float* ptr;
+  int ld, rows, cols;
+};
+
+struct FzParams {
+  int mode, post, B, kc1, n_src;
+  FzSrc src[4];
+  FzW w1, w2, w3, w4;
+  const float *b1, *b2, *gamma, *beta, *b3, *b4;
+  float eps;
+  int act1, has_gemm2;
+  const float* add[2];  // gathered GEMM1 addends (rows of 64): add[a][b * add_bs[a] + add_idx[a][r] * 64 + c]
+  const int32_t* add_idx[2];
+  long long add_bs[2];
+  const float* res;     // residual rows (64 wide)
+  long long res_bs;
+  float* out;           // (B, n_rows, out_w)
+  int out_w;
+  long long n_rows;
+  int n_tiles;
+  // EDGE
+  const int32_t* tile_rec;
+  const int32_t* rowptr;
+  int mean;
+  const float* edge;
+  long long edge_bs;
+  float* edge_out;      // (B, n_edges, 64) dense
+  float* aggr;          // (B, n_rec, 64) dense
+  long long n_rec, n_edges;
+  // POST_PROJ: out3 (B, n_rows, 64) = y·W3ᵀ, out4 = y·W4ᵀ + b4; POST_OUTMLP: y -> SiLU(y·W3ᵀ + b3) -> ·W4ᵀ + b4 -> step
+  float* out3;
+  float* out4;
+  // forecast-step epilogue on the final narrow output (width out_w)
+  int step;
+  const float *prev, *bnd, *mask, *dstd, *dmean;
+  // ROWLIN problem 1 (problem 0 = src[0], w1, b1, out, n_rows, n_tiles, B): weights in the W3 slot
+  FzSrc src1;
+  const float* b1_1;
+  float* out_1;
+  long long n_rows1;
+  int n_tiles1, B1;
+};
+
+// operands are rounded to TF32 (round to nearest) when written to shared memory; the MMA would otherwise drop the low
+// mantissa bits (a bias toward zero)
+__device__ __forceinline__ float tf32r(float x) {
+  uint32_t u;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
+  return __uint_as_float(u);
+}
+__device__ __forceinline__ float4 tf32r4(float4 v) { return make_float4(tf32r(v.x), tf32r(v.y), tf32r(v.z), tf32r(v.w)); }
+
+// byte offset of operand element (row R, column c) in a 128B-swizzled operand stored as 32-column chunks
+__device__ __forceinline__ uint32_t fz_off(uint32_t chunk_bytes, int R, int c) {
+  return (uint32_t)(c >> 5) * chunk_bytes + swz(R, (c & 31) >> 2) + (uint32_t)(c & 3) * 4;
+}
+
+__device__ void fz_load_w(uint8_t* s, const FzW& w, int kc, int tid) {
+  // rows 0..63 x 32*kc columns, zero past the real rows / columns
+  const int groups = 64 * kc * 8;
+  for (int g = tid; g < groups; g += fz::THREADS) {
+    const int n = g / (kc * 8), c = (g % (kc * 8)) * 4;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (w.ptr && n < w.rows) {
+      const float* p = w.ptr + (long long)n * w.ld + c;
+      if (c + 0 < w.cols) v.x = p[0];
+      if (c + 1 < w.cols) v.y = p[1];
+      if (c + 2 < w.cols) v.z = p[2];
+      if (c + 3 < w.cols) v.w = p[3];
+    }
+    *reinterpret_cast<float4*>(s + fz_off(fz::CH_W, n, c)) = tf32r4(v);
+  }
+}
+
+// A tile: rows row0 .. row0 + nrows - 1 of the concatenated sources (batch b), zero-padded to 32 * kc columns
+__device__ void fz_load_a(uint8_t* s, const FzSrc* src, int n_src, int kc, int b, long long row0, int nrows, int tid) {
+  const int gpr = kc * 8;
+  for (int g = tid; g < 128 * gpr; g += fz::THREADS) {
+    const int i = g / gpr, c = (g % gpr) * 4;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (i < nrows) {
+      const long long r = row0 + i;
+      float* pv = &v.x;
+      int off = 0;
+      for (int q = 0; q < n_src; ++q) {
+        const FzSrc& sq = src[q];
+        // vector load only for a whole group at a 16-byte aligned position of one source (rows of a width % 4 == 0)
+        if (c >= off && c + 4 <= off + sq.dim && ((c - off) & 3) == 0 && (sq.dim & 3) == 0) {
+          const long long rr = sq.idx ? (long long)__ldg(sq.idx + r) : r;
+          v = __ldg(reinterpret_cast<const float4*>(sq.ptr + b * sq.bs + rr * sq.dim + (c - off)));
+          break;
+        }
+        for (int e = 0; e < 4; ++e) {
+          const int cc = c + e - off;
+          if (cc >= 0 && cc < sq.dim) {
+            const long long rr = sq.idx ? (long long)__ldg(sq.idx + r) : r;
+            pv[e] = __ldg(sq.ptr + b * sq.bs + rr * sq.dim + cc);
+          }
+        }
+        off += sq.dim;
+      }
+    }
+    *reinterpret_cast<float4*>(s + fz_off(fz::CH_A, i, c)) = tf32r4(v);
+  }
+}
+
+// warp group MMA: acc (64 rows of this warp group x 64) = A[rows] · Wᵀ over kc chunks
+__device__ __forceinline__ void fz_gemm(float* acc, uint32_t a, uint32_t w, int kc) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  wgmma_fence(acc, 32);
+  for (int c = 0; c < kc; ++c) {
+    const uint64_t da = gmma_desc(a + c * fz::CH_A), db = gmma_desc(w + c * fz::CH_W);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) Wgmma<64>::mma(acc, da + 2 * k, db + 2 * k, (uint32_t)((c | k) != 0));
+  }
+  wgmma_commit();
+  wgmma_wait0(acc, 32);
+}
+
+// fragment of m64n64: acc[4j + 2i + e] is local row rq + 8i, column 8j + cq + e
+__device__ __forceinline__ void fz_unpack(const float* acc, float (*v)[16], const float* bias) {
+  const int cq = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) v[i][2 * j + e] = acc[4 * j + 2 * i + e] + (bias ? bias[8 * j + cq + e] : 0.f);
+}
+
+// this warp group's rows of v -> shared-memory operand (chunks 0-1 of A), then make them visible to its MMAs
+__device__ __forceinline__ void fz_store_op(uint8_t* sA, float (*v)[16], int rq, int wg) {
+  const int cq = 2 * (threadIdx.x & 3);
+  named_bar_sync(1 + wg, 128);  // every MMA of this warp group has finished reading the rows being replaced
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<float2*>(sA + fz_off(fz::CH_A, rq + 8 * i, 8 * j + cq)) =
+          make_float2(tf32r(v[i][2 * j]), tf32r(v[i][2 * j + 1]));
+  fence_proxy_async();
+  named_bar_sync(1 + wg, 128);
+}
+
+__device__ __forceinline__ void fz_layernorm(float (*v)[16], const float* gamma, const float* beta, float eps) {
+  const int cq = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float sm = 0.f, sq = 0.f;
+#pragma unroll
+    for (int t = 0; t < 16; ++t) {
+      sm += v[i][t];
+      sq = fmaf(v[i][t], v[i][t], sq);
+    }
+    sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+    sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+    sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+    sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+    const float mu = sm * (1.0f / 64), rstd = rsqrtf(fmaxf(sq * (1.0f / 64) - mu * mu, 0.f) + eps);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = 8 * j + cq + e;
+        v[i][2 * j + e] = fmaf((v[i][2 * j + e] - mu) * rstd, gamma[c], beta[c]);
+      }
+  }
+}
+
+// add 64-wide rows base[row(i)] (+ column offset of this thread) to v; row(i) < 0: skipped
+__device__ __forceinline__ void fz_add_rows(float (*v)[16], const float* p0, const float* p1) {
+  const int cq = 2 * (threadIdx.x & 3);
+  const float* p[2] = {p0, p1};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    if (!p[i]) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float2 x = __ldg(reinterpret_cast<const float2*>(p[i] + 8 * j + cq));
+      v[i][2 * j] += x.x;
+      v[i][2 * j + 1] += x.y;
+    }
+  }
+}
+
+// narrow / full-width row store with the optional forecast-step epilogue
+__device__ __forceinline__ void fz_store_rows(const FzParams& p, float* out, int W, long long n_rows, bool step, float (*v)[16],
+                                              int b, long long r0, bool valid0, bool valid1) {
+  const int cq = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    if (!(i ? valid1 : valid0)) continue;
+    const long long r = r0 + 8 * i;
+    const long long o = ((long long)b * n_rows + r) * W;
+    if (step) {
+      const float mk = p.bnd ? __ldg(p.mask + r) : 0.f;
+#pragma unroll
+      for (int t = 0; t < 16; ++t) {
+        const int c = 8 * (t >> 1) + cq + (t & 1);
+        if (c < W) {
+          const float nw = __ldg(p.prev + o + c) + (v[i][t] * __ldg(p.dstd + c) + __ldg(p.dmean + c));
+          out[o + c] = p.bnd ? mk * __ldg(p.bnd + o + c) + (1.f - mk) * nw : nw;
+        }
+      }
+    } else if (W == 64) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(out + o + 8 * j + cq) = make_float2(v[i][2 * j], v[i][2 * j + 1]);
+    } else {
+#pragma unroll
+      for (int t = 0; t < 16; ++t) {
+        const int c = 8 * (t >> 1) + cq + (t & 1);
+        if (c < W) out[o + c] = v[i][t];
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_constant__ FzParams p) {
+  using namespace fz;
+  const Layout L = layout(p.kc1, p.mode, p.post);
+  const uint32_t OFF_W1 = L.w1, OFF_W2 = L.w2, OFF_W3 = L.w3, OFF_W4 = L.w4, OFF_PRM = L.prm;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const uint32_t sb = smem_u32(s);
+  uint8_t* sA = s + OFF_A;
+  float* prm = reinterpret_cast<float*>(s + OFF_PRM);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2;
+  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // local row of fragment half 0 (half 1: + 8)
+  const int cq = 2 * (lane & 3);
+
+  fz_load_w(s + OFF_W1, p.w1, p.kc1, tid);
+  if (p.has_gemm2) fz_load_w(s + OFF_W2, p.w2, 2, tid);
+  if (p.post != POST_NONE || p.mode == ROWLIN) fz_load_w(s + OFF_W3, p.w3, 2, tid);
+  if (p.post != POST_NONE) fz_load_w(s + OFF_W4, p.w4, 2, tid);
+  for (int i = tid; i < 64; i += THREADS) {
+    prm[i] = p.b1 ? p.b1[i] : 0.f;
+    prm[64 + i] = p.b2 ? p.b2[i] : 0.f;
+    prm[128 + i] = p.gamma ? p.gamma[i] : 1.f;
+    prm[192 + i] = p.beta ? p.beta[i] : 0.f;
+    prm[256 + i] = p.b3 ? p.b3[i] : 0.f;
+    prm[320 + i] = p.b4 ? p.b4[i] : 0.f;
+    prm[384 + i] = p.b1_1 ? p.b1_1[i] : 0.f;
+  }
+  const long long n_work0 = (long long)p.n_tiles * p.B;
+  const long long n_work = n_work0 + (p.mode == ROWLIN ? (long long)p.n_tiles1 * p.B1 : 0);
+  float acc[32];
+  float v[2][16];
+  for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
+    // ------------------------------------------------------------------ which rows
+    int b, prob = 0;
+    long long t;
+    if (w < n_work0) {
+      b = (int)(w / p.n_tiles);
+      t = w - (long long)b * p.n_tiles;
+    } else {
+      prob = 1;
+      b = (int)((w - n_work0) / p.n_tiles1);
+      t = (w - n_work0) - (long long)b * p.n_tiles1;
+    }
+    long long row0;
+    int nrows;
+    if (p.mode == EDGE) {
+      const int ra = __ldg(p.tile_rec + t), rb = __ldg(p.tile_rec + t + 1);
+      row0 = __ldg(p.rowptr + ra);
+      nrows = __ldg(p.rowptr + rb) - (int)row0;
+    } else {
+      const long long n = prob ? p.n_rows1 : p.n_rows;
+      row0 = t * 128;
+      nrows = (int)min(128LL, n - row0);
+    }
+    __syncthreads();  // the previous tile's readers of the operand / message buffers are done
+    if (prob == 0) fz_load_a(sA, p.src, p.n_src, p.kc1, b, row0, nrows, tid);
+    else fz_load_a(sA, &p.src1, 1, p.kc1, b, row0, nrows, tid);
+    fence_proxy_async();
+    __syncthreads();
+    // ------------------------------------------------------------------ GEMM 1
+    fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + (prob ? OFF_W3 : OFF_W1), p.kc1);
+    const long long r0 = row0 + rq;
+    const bool valid0 = rq < nrows, valid1 = rq + 8 < nrows;
+    fz_unpack(acc, v, prm + (prob ? 384 : 0));
+    if (p.mode == ROWLIN) {
+      fz_store_rows(p, prob ? p.out_1 : p.out, 64, prob ? p.n_rows1 : p.n_rows, false, v, b, r0, valid0, valid1);
+      continue;
+    }
+    for (int a = 0; a < 2; ++a) {
+      if (!p.add[a]) continue;
+      const float* base = p.add[a] + (long long)b * p.add_bs[a];
+      fz_add_rows(v, valid0 ? base + (long long)__ldg(p.add_idx[a] + r0) * 64 : nullptr,
+                  valid1 ? base + (long long)__ldg(p.add_idx[a] + r0 + 8) * 64 : nullptr);
+    }
+    if (p.act1) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int t2 = 0; t2 < 16; ++t2) v[i][t2] = silu_fast(v[i][t2]);
+    }
+    // ------------------------------------------------------------------ GEMM 2
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W2, 2);
+    fz_unpack(acc, v, prm + 64);
+    if (p.gamma) fz_layernorm(v, prm + 128, prm + 192, p.eps);
+    if (p.mode == EDGE) {
+      // e' = e + m; m -> message buffer (row = local edge), then the per-receiver sums of the tile
+      if (p.edge_out) {
+        const float* e = p.edge + (long long)b * p.edge_bs;
+        float* eo = p.edge_out + (long long)b * p.n_edges * 64;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (!(i ? valid1 : valid0)) continue;
+          const long long k = r0 + 8 * i;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float2 x = *reinterpret_cast<const float2*>(e + k * 64 + 8 * j + cq);
+            *reinterpret_cast<float2*>(eo + k * 64 + 8 * j + cq) = make_float2(x.x + v[i][2 * j], x.y + v[i][2 * j + 1]);
+          }
+        }
+      }
+      float* msg = reinterpret_cast<float*>(s + OFF_W3);
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<float2*>(msg + (rq + 8 * i) * 64 + 8 * j + cq) = make_float2(v[i][2 * j], v[i][2 * j + 1]);
+      __syncthreads();
+      const int ra = __ldg(p.tile_rec + t), nrec = __ldg(p.tile_rec + t + 1) - ra;
+      for (int x = tid; x < nrec * 16; x += THREADS) {
+        const int rr = x >> 4, c4 = (x & 15) * 4;
+        const int k0 = __ldg(p.rowptr + ra + rr) - (int)row0, k1 = __ldg(p.rowptr + ra + rr + 1) - (int)row0;
+        float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int k = k0; k < k1; ++k) {
+          const float4 m = *reinterpret_cast<const float4*>(msg + k * 64 + c4);
+          sum.x += m.x; sum.y += m.y; sum.z += m.z; sum.w += m.w;
+        }
+        if (p.mean) {
+          const float sc = 1.f / (float)max(k1 - k0, 1);
+          sum.x *= sc; sum.y *= sc; sum.z *= sc; sum.w *= sc;
+        }
+        *reinterpret_cast<float4*>(p.aggr + ((long long)b * p.n_rec + ra + rr) * 64 + c4) = sum;
+      }
+      continue;
+    }
+    if (p.res) {
+      const float* base = p.res + (long long)b * p.res_bs;
+      fz_add_rows(v, valid0 ? base + r0 * 64 : nullptr, valid1 ? base + (r0 + 8) * 64 : nullptr);
+    }
+    if (p.post == POST_NONE) {
+      fz_store_rows(p, p.out, p.out_w, p.n_rows, p.step, v, b, r0, valid0, valid1);
+      continue;
+    }
+    if (p.post == POST_PROJ) {
+      fz_store_rows(p, p.out, 64, p.n_rows, false, v, b, r0, valid0, valid1);  // the updated node rows
+      fz_store_op(sA, v, rq, wg);
+      fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W3, 2);
+      fz_unpack(acc, v, nullptr);
+      fz_store_rows(p, p.out3, 64, p.n_rows, false, v, b, r0, valid0, valid1);
+      fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W4, 2);
+      fz_unpack(acc, v, prm + 320);
+      fz_store_rows(p, p.out4, 64, p.n_rows, false, v, b, r0, valid0, valid1);
+      continue;
+    }
+    // POST_OUTMLP: the updated node rows stay on chip
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W3, 2);
+    fz_unpack(acc, v, prm + 256);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t2 = 0; t2 < 16; ++t2) v[i][t2] = silu_fast(v[i][t2]);
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W4, 2);
+    fz_unpack(acc, v, prm + 320);
+    fz_store_rows(p, p.out, p.out_w, p.n_rows, true, v, b, r0, valid0, valid1);
+  }
+}
+
+// ------------------------------------------------------------------------------------ host
+static FzW wslice(const float* w, int ld, int rows, int cols) { return FzW{w, ld, rows, cols}; }
+
+static int fz_launch(const FzParams& p, const char* name, double bytes, cudaStream_t st) {
+  const long long n_work = (long long)p.n_tiles * p.B + (p.mode == fz::ROWLIN ? (long long)p.n_tiles1 * p.B1 : 0);
+  if (n_work == 0) return NLAM_OK;
+  NLAM_REQUIRE(n_work < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  const size_t smem = fz::layout(p.kc1, p.mode, p.post).bytes;
+  static unsigned mask = 0;
+  if (!(mask & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(fused_mlp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)fz::layout(6, fz::EDGE, 0).bytes));
+    mask |= 1u << (dev & 31);
+  }
+  int per_sm = 1;
+  NLAM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fused_mlp_kernel, fz::THREADS, smem));
+  const int grid = (int)std::min<long long>(n_work, (long long)num_sms() * std::max(per_sm, 1));
+  {
+    ProfScope ps(name, st, bytes);
+    fused_mlp_kernel<<<grid, fz::THREADS, smem, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
+}
+
+static void fz_mlp(FzParams& p, const NlamMlp* m, int k_off, int k_cols) {
+  // first Linear: columns [k_off, k_off + k_cols) of w[0]; second Linear + LayerNorm
+  p.w1 = wslice(m->w[0] + k_off, m->in_dim, 64, k_cols);
+  p.kc1 = (k_cols + 31) / 32;
+  p.b1 = m->b[0];
+  p.act1 = 1;
+  p.has_gemm2 = 1;
+  p.w2 = wslice(m->w[1], 64, m->out_dim[1], 64);
+  p.b2 = m->b[1];
+  p.gamma = m->ln_gamma;
+  p.beta = m->ln_beta;
+  p.eps = m->ln_eps;
+}
+
+// ---- row MLPs (H = 64): embedders, node updates, output_map (+ step epilogue)
+bool tc_rowmlp_supported(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res, const NlamRowSrc* res2,
+                         int64_t n_rows) {
+  int nout = 0;
+  if (res2 || n_rows < 1 || n_rows >= (1LL << 31) - 256 || n_src < 1 || n_src > 4) return false;
+  if (!mlp_shape_ok(mlp, &nout)) return false;
+  int k = 0;
+  for (int s = 0; s < n_src; ++s) {
+    if (srcs[s].idx || !aligned16(srcs[s].ptr) || srcs[s].bstride % 4 != 0) return false;
+    k += srcs[s].dim;
+  }
+  if (k != mlp->in_dim) return false;
+  bool all_wide = n_src <= 2;
+  for (int s = 0; s < n_src; ++s) all_wide = all_wide && srcs[s].dim == 64;
+  if (all_wide) {  // node updates / encoders: the residual is one of the inputs
+    if (res) {
+      if (nout != 64 || res->idx) return false;
+      bool match = false;
+      for (int s = 0; s < n_src; ++s) match = match || (srcs[s].ptr == res->ptr && srcs[s].bstride == res->bstride);
+      if (!match) return false;
+    }
+    return true;
+  }
+  // narrow concatenation (grid embedder, output_map inputs): total width <= 64, no residual
+  return !res && mlp->in_dim <= 64;
+}
+
+int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res, float* out, int64_t n_rows, int B,
+              cudaStream_t st, const StepEpilogue* ep) {
+  NLAM_REQUIRE(tc_rowmlp_supported(mlp, srcs, n_src, res, nullptr, n_rows), NLAM_E_UNSUPPORTED, "tc_rowmlp: unsupported shape");
+  const int nout = mlp->out_dim[1];
+  NLAM_REQUIRE(!ep || (nout < 64 && !mlp->ln_gamma && !res), NLAM_E_UNSUPPORTED,
+               "tc_rowmlp: the fused step epilogue needs a narrow output without LayerNorm / residual");
+  FzParams p;
+  memset(&p, 0, sizeof(p));
+  p.mode = fz::ROWS;
+  p.B = B;
+  p.n_src = n_src;
+  double bytes = 0;
+  for (int s = 0; s < n_src; ++s) {
+    p.src[s] = FzSrc{srcs[s].ptr, srcs[s].idx, B > 1 ? srcs[s].bstride : 0, srcs[s].dim};
+    bytes += 4.0 * n_rows * srcs[s].dim * ((srcs[s].bstride != 0 && B > 1) ? B : 1);
+  }
+  fz_mlp(p, mlp, 0, mlp->in_dim);
+  if (res) {
+    p.res = res->ptr;
+    p.res_bs = B > 1 ? res->bstride : 0;
+    bytes += 4.0 * n_rows * 64 * ((res->bstride != 0 && B > 1) ? B : 1);
+  }
+  p.out = out;
+  p.out_w = nout;
+  p.n_rows = n_rows;
+  p.n_tiles = (int)((n_rows + 127) / 128);
+  bytes += 4.0 * n_rows * B * nout;
+  if (ep) {
+    p.step = 1;
+    p.prev = ep->prev;
+    p.bnd = ep->boundary;
+    p.mask = ep->mask;
+    p.dstd = ep->std;
+    p.dmean = ep->mean;
+    bytes += 4.0 * n_rows * B * nout * (ep->boundary ? 2 : 1);
+  }
+  return fz_launch(p, "tc_rowmlp_kernel", bytes, st);
+}
+
+// ---- node projections of the split first edge Linear: P_s = x_s·W1sᵀ (B_s batches), P_r = x_r·W1rᵀ + b1 (B_r batches)
+static int fz_projections(const NlamGraph* g, const NlamMlp* em, const float* send, int64_t send_bs, const float* rec,
+                          int64_t rec_bs, int B, float* Ps, float* Pr, cudaStream_t st) {
+  const int Bs = (send_bs == 0 || B == 1) ? 1 : B, Br = (rec_bs == 0 || B == 1) ? 1 : B;
+  FzParams p;
+  memset(&p, 0, sizeof(p));
+  p.mode = fz::ROWLIN;
+  p.n_src = 1;
+  p.src[0] = FzSrc{send, nullptr, Bs > 1 ? send_bs : 0, 64};
+  p.w1 = wslice(em->w[0] + 64, 192, 64, 64);
+  p.kc1 = 2;
+  p.out = Ps;
+  p.out_w = 64;
+  p.n_rows = g->n_send;
+  p.n_tiles = (int)((g->n_send + 127) / 128);
+  p.B = Bs;
+  p.src1 = FzSrc{rec, nullptr, Br > 1 ? rec_bs : 0, 64};
+  p.w3 = wslice(em->w[0] + 128, 192, 64, 64);
+  p.b1_1 = em->b[0];
+  p.out_1 = Pr;
+  p.n_rows1 = g->n_rec;
+  p.n_tiles1 = (int)((g->n_rec + 127) / 128);
+  p.B1 = Br;
+  return fz_launch(p, "tc_rowlinear_kernel", 8.0 * 64 * ((double)g->n_send * Bs + (double)g->n_rec * Br), st);
+}
+
+// ---- edge stage: messages, optional edge output, per-receiver aggregate
+bool tc_edge_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags) {
+  int nout = 0;
+  if (flags & NLAM_PROPAGATION) return false;
+  if (!g || g->n_tiles <= 0) return false;
+  if (!mlp_shape_ok(edge_mlp, &nout) || nout != 64 || edge_mlp->in_dim != 192 || !edge_mlp->ln_gamma) return false;
+  return true;
+}
+
+static int edge_mode_env() {
+  // NLAM_TC_EDGE=v1 | v2 forces one formulation of the first edge Linear
+  static int mode = -1;
+  if (mode < 0) {
+    const char* e = getenv("NLAM_TC_EDGE");
+    mode = (e && e[0] == 'v' && e[1] == '1') ? 1 : (e && e[0] == 'v' && e[1] == '2') ? 2 : 0;
+  }
+  return mode;
+}
+
+bool tc_edge2_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
+                        const float* rec, int64_t rec_bs, int B, int64_t send_rows) {
+  (void)send_rows;
+  // default: the split form (node projections + K = 64 edge GEMM) where the per-node projection pass is small next to the
+  // edge work (mesh graph: ~9 edges per node); the K = 192 form otherwise (grid -> mesh)
+  const int mode = edge_mode_env();
+  if (mode == 1) return false;
+  if (!tc_edge_supported(g, edge_mlp, flags)) return false;
+  if (!(aligned16(send) && aligned16(rec) && send_bs % 4 == 0 && rec_bs % 4 == 0)) return false;
+  if (mode == 2) return true;
+  const double edge_rows = (double)g->n_edges * B;
+  const double node_rows = (double)g->n_send * ((send_bs == 0 || B == 1) ? 1 : B) +
+                           (double)g->n_rec * ((rec_bs == 0 || B == 1) ? 1 : B);
+  return edge_rows >= 2.5 * node_rows;
+}
+
+size_t tc_edge2_workspace_floats(const NlamGraph* g, int B, int64_t send_rows_max) {
+  (void)send_rows_max;
+  return (size_t)B * (size_t)(g->n_send + g->n_rec) * 64 + 64;
+}
+
+bool tc_edge_bcast_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
+                             const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B, bool has_edge_out) {
+  if (has_edge_out || !tc_edge_supported(g, edge_mlp, flags)) return false;
+  if (!(edge_bs == 0 || B == 1) || !(rec_bs == 0 || B == 1)) return false;  // edge features and receivers shared by the batch
+  return aligned16(send) && aligned16(rec) && aligned16(edge) && send_bs % 4 == 0;
+}
+
+bool tc_ell_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
+                      const float* rec, int64_t rec_bs, bool has_edge_out) {
+  if (has_edge_out || !g || g->uniform_degree < 1 || g->uniform_degree > 8 || !g->ell_window) return false;
+  if (!tc_edge_supported(g, edge_mlp, flags)) return false;
+  return aligned16(send) && aligned16(rec) && send_bs % 4 == 0 && rec_bs % 4 == 0;
+}
+
+bool tc_edge_rmw_supported(const NlamGraph* g, const float* edge, int64_t edge_bs, const float* edge_out, int B) {
+  if (!edge_out) return true;
+  return edge_out == edge && (B == 1 || edge_bs == (int64_t)g->n_edges * 64);
+}
+
+// split: A = e, + P_s[src] + P_r[dst] in the GEMM 1 epilogue (projections in ws, or from the previous layer when have_proj);
+// otherwise A = [e | x_src | x_dst] (K = 192)
+static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
+                   const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st,
+                   float* ws, bool split, bool have_proj, const char* name) {
+  NLAM_REQUIRE(tc_edge_supported(g, em, flags), NLAM_E_UNSUPPORTED, "%s: unsupported shape", name);
+  NLAM_REQUIRE(aligned16(send) && aligned16(rec) && aligned16(edge) && aligned16(aggr_out) && (!edge_out || aligned16(edge_out)) &&
+                   send_bs % 4 == 0 && rec_bs % 4 == 0 && edge_bs % 4 == 0,
+               NLAM_E_INVALID, "%s: pointers / strides must be 16-byte aligned", name);
+  const int Bs = (send_bs == 0 || B == 1) ? 1 : B, Br = (rec_bs == 0 || B == 1) ? 1 : B;
+  const int64_t eb = B > 1 ? edge_bs : 0;
+  FzParams p;
+  memset(&p, 0, sizeof(p));
+  p.mode = fz::EDGE;
+  p.B = B;
+  if (split) {
+    float* Ps = ws;
+    float* Pr = ws + (size_t)(have_proj ? B : Bs) * g->n_send * 64;
+    if (!have_proj) {
+      int rc = fz_projections(g, em, send, send_bs, rec, rec_bs, B, Ps, Pr, st);
+      if (rc) return rc;
+    }
+    p.n_src = 1;
+    p.src[0] = FzSrc{edge, nullptr, eb, 64};
+    fz_mlp(p, em, 0, 64);
+    p.b1 = nullptr;  // carried by P_r
+    p.add[0] = Ps;
+    p.add_idx[0] = g->src;
+    p.add_bs[0] = (have_proj ? B : Bs) > 1 ? g->n_send * 64 : 0;
+    p.add[1] = Pr;
+    p.add_idx[1] = g->dst;
+    p.add_bs[1] = (have_proj ? B : Br) > 1 ? g->n_rec * 64 : 0;
+  } else {
+    p.n_src = 3;
+    p.src[0] = FzSrc{edge, nullptr, eb, 64};
+    p.src[1] = FzSrc{send, g->src, Bs > 1 ? send_bs : 0, 64};
+    p.src[2] = FzSrc{rec, g->dst, Br > 1 ? rec_bs : 0, 64};
+    fz_mlp(p, em, 0, 192);
+  }
+  p.n_tiles = g->n_tiles;
+  p.tile_rec = g->tile_rec;
+  p.rowptr = g->rowptr;
+  p.mean = (flags & NLAM_AGGR_MEAN) ? 1 : 0;
+  p.edge = edge;
+  p.edge_bs = eb;
+  p.edge_out = edge_out;
+  p.aggr = aggr_out;
+  p.n_rec = g->n_rec;
+  p.n_edges = g->n_edges;
+  return fz_launch(p, name, edge_algorithmic_bytes(g, B, send_bs, rec_bs, edge_bs, edge_out != nullptr, 64), st);
+}
+
+int tc_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
+            const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st,
+            int64_t send_rows) {
+  (void)send_rows;
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, nullptr, false, false,
+                 "tc_edge_kernel");
+}
+
+int tc_edge3(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
+             const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
+             bool have_proj) {
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, ws, true, have_proj,
+                 "tc_edge3_kernel");
+}
+
+int tc_edge_rmw(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
+                const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
+                bool have_proj) {
+  NLAM_REQUIRE(!edge_out || edge_out == edge, NLAM_E_INVALID, "tc_edge_rmw: the edge output must alias the edge input");
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, ws, true, have_proj,
+                 "tc_edge_rmw_kernel");
+}
+
+int tc_ell_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
+                const float* edge, int64_t edge_bs, float* aggr_out, int B, int flags, cudaStream_t st, float* ws) {
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, nullptr, aggr_out, B, flags, st, ws, true, false,
+                 "tc_ell_window_kernel");
+}
+
+int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
+                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws) {
+  // split form: the batch-shared receiver projection is computed once, the sender projection once per node (both far fewer
+  // rows than the batch's edges), and the edge GEMM has K = 64 instead of gathering K = 192 raw rows per edge and batch
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, 0, nullptr, aggr_out, B, flags, st, ws, true, false,
+                 "tc_edge_bcast_kernel");
+}
+
+// ---- node update chained with the next layer's projections / with output_map + step epilogue
+static bool node_mlp_ok(const NlamMlp* m) {
+  int no = 0;
+  return mlp_shape_ok(m, &no) && no == 64 && m->in_dim == 128 && m->ln_gamma && m->ln_beta;
+}
+
+bool tc_node_proj_supported(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs,
+                            const float* aggr, int64_t n_rows, const float* out, const float* proj_out) {
+  int no2 = 0;
+  if (n_rows < 1 || n_rows >= (1LL << 31) - 256 || !node_mlp_ok(node_mlp)) return false;
+  if (!mlp_shape_ok(next_edge_mlp, &no2) || no2 != 64 || next_edge_mlp->in_dim != 192) return false;
+  return aligned16(rec) && aligned16(aggr) && aligned16(out) && aligned16(proj_out) && rec_bs % 4 == 0;
+}
+
+static void fz_node(FzParams& p, const NlamMlp* node_mlp, const float* rec, int64_t rec_bs, const float* aggr, int64_t n_rows,
+                    int B) {
+  p.mode = fz::ROWS;
+  p.B = B;
+  p.n_src = 2;
+  p.src[0] = FzSrc{rec, nullptr, B > 1 ? rec_bs : 0, 64};
+  p.src[1] = FzSrc{aggr, nullptr, B > 1 ? n_rows * 64 : 0, 64};
+  fz_mlp(p, node_mlp, 0, 128);
+  p.res = rec;
+  p.res_bs = B > 1 ? rec_bs : 0;
+  p.n_rows = n_rows;
+  p.n_tiles = (int)((n_rows + 127) / 128);
+}
+
+int tc_node_proj(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs, const float* aggr,
+                 int64_t n_rows, int B, float* out, float* proj_out, cudaStream_t st) {
+  NLAM_REQUIRE(tc_node_proj_supported(node_mlp, next_edge_mlp, rec, rec_bs, aggr, n_rows, out, proj_out), NLAM_E_UNSUPPORTED,
+               "tc_node_proj: unsupported shapes");
+  FzParams p;
+  memset(&p, 0, sizeof(p));
+  fz_node(p, node_mlp, rec, rec_bs, aggr, n_rows, B);
+  p.post = fz::POST_PROJ;
+  p.out = out;
+  p.out_w = 64;
+  p.w3 = wslice(next_edge_mlp->w[0] + 64, 192, 64, 64);
+  p.w4 = wslice(next_edge_mlp->w[0] + 128, 192, 64, 64);
+  p.b4 = next_edge_mlp->b[0];
+  p.out3 = proj_out;
+  p.out4 = proj_out + (size_t)B * n_rows * 64;
+  return fz_launch(p, "tc_node_proj_kernel", 4.0 * n_rows * 64 * (((rec_bs != 0 && B > 1) ? B : 1) + 4.0 * B), st);
+}
+
+bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
+                           int64_t n_rows, int B, const float* out, const StepEpilogue* ep) {
+  int no2 = 0;
+  (void)B;
+  if (n_rows < 1 || n_rows >= (1LL << 31) - 256 || !node_mlp_ok(node_mlp)) return false;
+  if (!mlp_shape_ok(out_mlp, &no2) || no2 >= 64 || out_mlp->in_dim != 64 || out_mlp->ln_gamma) return false;
+  if (!(aligned16(rec) && aligned16(aggr) && rec_bs % 4 == 0 && out)) return false;
+  return ep && ep->prev && ep->std && ep->mean && (!ep->boundary || ep->mask);
+}
+
+int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
+                int64_t n_rows, int B, float* out, const StepEpilogue* ep, cudaStream_t st) {
+  NLAM_REQUIRE(tc_node_out_supported(node_mlp, out_mlp, rec, rec_bs, aggr, n_rows, B, out, ep), NLAM_E_UNSUPPORTED,
+               "tc_node_out: unsupported shapes");
+  FzParams p;
+  memset(&p, 0, sizeof(p));
+  fz_node(p, node_mlp, rec, rec_bs, aggr, n_rows, B);
+  const int D = out_mlp->out_dim[1];
+  p.post = fz::POST_OUTMLP;
+  p.w3 = wslice(out_mlp->w[0], 64, 64, 64);
+  p.b3 = out_mlp->b[0];
+  p.w4 = wslice(out_mlp->w[1], 64, D, 64);
+  p.b4 = out_mlp->b[1];
+  p.out = out;
+  p.out_w = D;
+  p.step = 1;
+  p.prev = ep->prev;
+  p.bnd = ep->boundary;
+  p.mask = ep->mask;
+  p.dstd = ep->std;
+  p.dmean = ep->mean;
+  return fz_launch(p, "tc_node_out_kernel", 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + 3.0 * D * B), st);
+}
+
+}  // namespace nlam

@@ -113,7 +113,7 @@ extern "C" int nlam_abi_version(void) { return NLAM_ABI_VERSION; }
 extern "C" const char* nlam_last_error(void) { return nlam::get_error(); }
 extern "C" int64_t nlam_launch_count(void) { return nlam::launch_count(); }
 extern "C" const char* nlam_build_info(void) {
-  return "libnlam_b200 abi=1 arch=sm_100a cuda=" __DATE__;
+  return "libnlam_b200 abi=1 arch=sm_90a cuda=" __DATE__;
 }
 
 template <class T>
@@ -195,72 +195,8 @@ extern "C" int nlam_graph_create(NlamGraph** out, const int64_t* edge_index, int
     }
     g->n_tiles = (int32_t)tile_rec.size() - 1;
   }
-  std::vector<int32_t> tile_e0(tile_rec.size());
-  for (size_t i = 0; i < tile_rec.size(); ++i) tile_e0[i] = rowptr[tile_rec[i]];
-  std::vector<int32_t> tile_meta;
-  for (size_t i = 0; i + 1 < tile_rec.size(); ++i) {
-    tile_meta.push_back(tile_e0[i]);
-    tile_meta.push_back(tile_e0[i + 1] - tile_e0[i]);
-    tile_meta.push_back(tile_rec[i]);
-    tile_meta.push_back(tile_rec[i + 1] - tile_rec[i]);
-  }
-  // sender windows of the CSR tiles (tc2.cu): tile t works on the 128-edge window [e0, e0+128) (the edges past
-  // its own are recomputed identically by the following tiles), which reads <= 128 distinct senders
-  std::vector<int32_t> win_u, win_nu;
-  std::vector<uint8_t> win_loc;
-  if (g->n_tiles > 0) {
-    const int64_t nt = g->n_tiles;
-    win_u.assign((size_t)nt * 128, 0);
-    win_nu.assign((size_t)nt, 0);
-    win_loc.assign((size_t)nt * 128, 0);
-    std::vector<int32_t> u;
-    for (int64_t t = 0; t < nt; ++t) {
-      const int64_t k0 = tile_e0[t], k1 = std::min<int64_t>(E, k0 + 128);
-      if (k1 <= k0) continue;
-      u.assign(src.begin() + k0, src.begin() + k1);
-      std::sort(u.begin(), u.end());
-      u.erase(std::unique(u.begin(), u.end()), u.end());
-      for (int64_t k = k0; k < k1; ++k)
-        win_loc[(size_t)t * 128 + (k - k0)] = (uint8_t)(std::lower_bound(u.begin(), u.end(), src[k]) - u.begin());
-      const size_t nu = (u.size() + 3) / 4 * 4;
-      for (size_t i = 0; i < nu; ++i) win_u[(size_t)t * 128 + i] = u[std::min(i, u.size() - 1)];
-      win_nu[t] = (int32_t)nu;
-    }
-  }
-  // Receiver tiles + sender windows of the ELL kernel (tc3.cu): a tile is up to 128 CONSECUTIVE receivers whose d*nrec
-  // edges read at most 128 distinct senders (the window); a tile is cut short where the next receivers would overflow the
-  // window (mesh->grid on a 268 x 238 grid: a 128-receiver block that wraps around a grid row reads up to 135 mesh nodes),
-  // so every uniform-degree edge set has a tiling.
-  std::vector<int32_t> ell_u, ell_nu, ell_r0;
-  std::vector<uint8_t> ell_loc;
-  if (g->uniform_degree >= 1 && g->uniform_degree <= 8) {
-    const int64_t d = g->uniform_degree;
-    ell_loc.assign((size_t)E, 0);
-    std::vector<int32_t> u;
-    int64_t r0 = 0;
-    while (r0 < n_rec) {
-      int64_t nrec = std::min<int64_t>(128, n_rec - r0);
-      for (;;) {
-        u.assign(src.begin() + d * r0, src.begin() + d * (r0 + nrec));
-        std::sort(u.begin(), u.end());
-        u.erase(std::unique(u.begin(), u.end()), u.end());
-        if (u.size() <= 128) break;
-        nrec -= (nrec > 16) ? 8 : 1;  // 8 receivers of degree <= 8 always fit
-      }
-      for (int64_t k = d * r0; k < d * (r0 + nrec); ++k)
-        ell_loc[k] = (uint8_t)(std::lower_bound(u.begin(), u.end(), src[k]) - u.begin());
-      const size_t nu = (u.size() + 3) / 4 * 4;
-      const size_t base = ell_u.size();
-      ell_u.resize(base + 128, 0);
-      for (size_t i = 0; i < nu; ++i) ell_u[base + i] = u[std::min(i, u.size() - 1)];
-      ell_nu.push_back((int32_t)nu);
-      ell_r0.push_back((int32_t)r0);
-      r0 += nrec;
-    }
-    ell_r0.push_back((int32_t)n_rec);
-    g->ell_window = 1;
-    g->ell_nt = (int32_t)ell_nu.size();
-  }
+  // uniform in-degree edge sets of degree <= 8 (mesh -> grid, mesh-down) take the uniform-degree edge path
+  if (g->uniform_degree >= 1 && g->uniform_degree <= 8) g->ell_window = 1;
   g->h_tile_rec = tile_rec;
   g->h_rowptr = rowptr;
 
@@ -281,10 +217,7 @@ extern "C" int nlam_graph_create(NlamGraph** out, const int64_t* edge_index, int
   if ((rc = upload(&g->rowptr, rowptr)) || (rc = upload(&g->src, src)) || (rc = upload(&g->dst, dst)) ||
       (rc = upload(&g->perm, perm)) || (rc = upload(&g->inv_perm, inv_perm)) ||
       (rc = upload(&g->sptr, sptr)) || (rc = upload(&g->sperm, sperm)) ||
-      (rc = upload(&g->tile_rec, tile_rec)) || (rc = upload(&g->tile_e0, tile_e0)) ||
-      (rc = upload(&g->tile_meta, tile_meta)) || (rc = upload(&g->ell_u, ell_u)) ||
-      (rc = upload(&g->ell_nu, ell_nu)) || (rc = upload(&g->ell_loc, ell_loc)) || (rc = upload(&g->ell_r0, ell_r0)) ||
-      (rc = upload(&g->win_u, win_u)) || (rc = upload(&g->win_nu, win_nu)) || (rc = upload(&g->win_loc, win_loc))) {
+      (rc = upload(&g->tile_rec, tile_rec))) {
     cudaSetDevice(prev_dev);
     nlam_graph_destroy(g);
     return rc;
@@ -307,15 +240,6 @@ extern "C" void nlam_graph_destroy(NlamGraph* g) {
   cudaFree(g->sptr);
   cudaFree(g->sperm);
   cudaFree(g->tile_rec);
-  cudaFree(g->tile_e0);
-  cudaFree(g->tile_meta);
-  cudaFree(g->ell_u);
-  cudaFree(g->ell_nu);
-  cudaFree(g->ell_loc);
-  cudaFree(g->ell_r0);
-  cudaFree(g->win_u);
-  cudaFree(g->win_nu);
-  cudaFree(g->win_loc);
   cudaSetDevice(prev);
   delete g;
 }

@@ -7,7 +7,7 @@
 //   gather_rows      x.index_select(-2, idx) (PyG propagate, gnn_layers.py:145)
 //   step_epilogue    rescale + residual + boundary mix (graph/base.py:339-342,
 //                    forecasters/autoregressive.py:128-131)
-// These are the "exact" path and the fallback for shapes the tcgen05 kernels do not cover.
+// These are the "exact" path and the fallback for shapes the tensor-core kernels do not cover.
 #include "common.cuh"
 
 namespace nlam {
@@ -274,7 +274,7 @@ int rowmlp_simt(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const Nla
   long long n_work = (long long)p.tiles_per_batch * B;
   NLAM_CUDA_OK(cudaFuncSetAttribute(rowmlp_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = std::max<int>(1, (int)((220 * 1024) / (smem + 1024)));
-  int grid = (int)std::min<long long>(n_work, (long long)148 * std::min(occ, 4));
+  int grid = (int)std::min<long long>(n_work, (long long)132 * std::min(occ, 4));
   {
     ProfScope ps("rowmlp_simt_kernel", stream, rowmlp_algorithmic_bytes(mlp, srcs, n_src, res, res2, n_rows, B, out2 != nullptr, nullptr));
     rowmlp_simt_kernel<<<grid, NT, smem, stream>>>(p);
@@ -413,7 +413,7 @@ __global__ void step_epilogue_clamped_kernel(const float* __restrict__ net_out, 
 
 static int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  return (int)std::max<long long>(1, std::min<long long>(g, 148LL * 16));
+  return (int)std::max<long long>(1, std::min<long long>(g, 132LL * 16));
 }
 
 }  // namespace nlam

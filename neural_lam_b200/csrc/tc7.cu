@@ -1,26 +1,26 @@
-// Generic tcgen05 Linear kernel for hidden widths the fused H = 64 kernels do not cover (H = 128 / 256: BASELINE
-// configs 3-5), and for the layer variants they do not cover at H = 64 (PropagationNet):
+// Generic tensor-core Linear kernel (sm_90a: wgmma TF32) for hidden widths and layer variants the fused kernels do not
+// cover:
 //
 //     Y[r, :] = epi( [X0 | X1][r, :] · Wᵀ + bias + A0[idx0[r], :] + A1[idx1[r], :] )
-//     epi: none | SiLU | LayerNorm (two passes over the TMEM accumulator), then "+ post[idxp[r]]" (PropagationNet's
-//     x_j + edge_mlp(...)), a second output before the residual (the message m next to e' = e + m) and "+ residual".
+//     epi: none | SiLU | LayerNorm, then "+ post[idxp[r]]" (PropagationNet's x_j + edge_mlp(...)), a second output before
+//     the residual (the message m next to e' = e + m) and "+ residual".
 //
-// One CTA tile = 128 rows x N (N = the full output width <= 256 = one UMMA instruction shape M128 x N), K streamed
-// in 32-column chunks through a ring of shared-memory stages: the X chunk (16 KB) and the W chunk (N x 128 B, L2
-// resident) arrive by TMA, `tcgen05.mma kind::tf32` accumulates into one of TWO TMEM accumulator buffers (2 x N <= 512
-// columns), so that the epilogue of tile i (128 threads, thread = row, `tcgen05.ld` 32 columns at a time) overlaps the
-// GEMM of tile i + 1.  Warp roles: 0 = TMA producer, 1 = MMA issue, 2-5 = epilogue.
+// One CTA tile = 128 rows x N (N = the full output width <= 256), K streamed in 32-column chunks through a ring of
+// shared-memory stages: the X chunk (16 KB) and the W chunk (N x 128 B, L2 resident) arrive by TMA with 128-byte swizzle,
+// and two consumer warp groups each run `wgmma.mma_async m64nNk8 .tf32` on their 64 rows of the stage, accumulating in
+// registers; the epilogue works on the accumulator fragments (a row is spread over the 4 threads of a quad; LayerNorm
+// statistics are reduced with two shuffles).  Warp group 0 is the TMA producer.
 // An MLP (reference utils/networks.py:27-40) is two launches with the hidden activations in a workspace; an
 // InteractionNet (reference gnn_layers.py:110-157) is: node projections of the split first edge Linear, edge layer 1
 // (gathered projections added in the epilogue, SiLU), edge layer 2 (LayerNorm, m and e' = e + m), CSR segment sum,
-// node layers 1 / 2.  At H = 256 the path is tensor-pipe bound (SURVEY 8d), which is what this kernel is for; the
-// fully fused H = 64 kernels (tc3-tc6) stay the path of the BASELINE metric.
+// node layers 1 / 2.
 #include "tc_ptx.cuh"
+#include "wgmma_tf32.cuh"
 
 namespace nlam {
 
 namespace g7 {
-constexpr int THREADS = 192;
+constexpr int THREADS = 384;           // warp group 0: TMA producer (one thread); warp groups 1 / 2: rows 0-63 / 64-127
 constexpr int KC = 32;                 // K columns per chunk (128 bytes: one swizzle row)
 constexpr uint32_t A_BYTES = 128 * 128;  // 128 rows x 128 B
 }  // namespace g7
@@ -54,6 +54,15 @@ struct LinParams {
   int stages;
 };
 
+__device__ __forceinline__ void add_row2(float* v, const float* row, int N) {
+  // v[2j + e] += row[8j + e]: the column pairs one thread holds of a row (row already offset by 2 * (lane & 3))
+  for (int j = 0; j < N / 8; ++j) {
+    const float2 x = __ldg(reinterpret_cast<const float2*>(row + 8 * j));
+    v[2 * j] += x.x;
+    v[2 * j + 1] += x.y;
+  }
+}
+
 template <int N>
 __global__ void __launch_bounds__(g7::THREADS, 1)
 tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
@@ -61,43 +70,27 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   using namespace g7;
   constexpr uint32_t W_BYTES = N * 128;
   constexpr uint32_t STG_BYTES = A_BYTES + W_BYTES;
-  constexpr uint32_t TM_COLS = (2 * N <= 32) ? 32 : (2 * N <= 64) ? 64 : (2 * N <= 128) ? 128 : (2 * N <= 256) ? 256 : 512;
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int wg = warp >> 2;
   const int NSTG = p.stages;
   const uint32_t off_misc = (uint32_t)NSTG * STG_BYTES;
   const uint32_t mb = sbase + off_misc;
-  const uint32_t bar_full = mb;             // [8]
-  const uint32_t bar_empty = mb + 64;       // [8]
-  const uint32_t bar_acc_full = mb + 128;   // [2]
-  const uint32_t bar_acc_empty = mb + 144;  // [2] 128 arrivals
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + off_misc + 160);
+  const uint32_t bar_full = mb;        // [8] TMA bytes landed
+  const uint32_t bar_empty = mb + 64;  // [8] 8 arrivals: every consumer warp has finished its MMAs on the stage
   float* sprm = reinterpret_cast<float*>(smem + off_misc + 256);  // bias | gamma | beta (N each)
   if ((sbase & 1023u) != 0) {
     if (tid == 0) printf("nlam tc_linear: dynamic shared memory not 1024-byte aligned\n");
     __trap();
   }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < NSTG; ++s) {
-        mbar_init(bar_full + 8 * s, 1);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(bar_acc_full + 8 * s, 1);
-        mbar_init(bar_acc_empty + 8 * s, 128);
-      }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (tid == 0) {
+    for (int s = 0; s < NSTG; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 8);
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"(TM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp == 0 && lane == 0) {
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA0) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA1) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
@@ -107,16 +100,13 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
     sprm[N + i] = p.gamma ? p.gamma[i] : 1.f;
     sprm[2 * N + i] = p.beta ? p.beta[i] : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_ptr_smem, 0);
   const long long n_work = (long long)p.n_tiles * p.B;
   const int kc_total = p.kc0 + p.kc1;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // =============================== TMA producer ===============================
-    if (lane == 0) {
+    if (tid == 0) {
       const uint64_t pol_stream = policy_evict_first();
       const uint64_t pol_keep = policy_evict_last();
       long long c = 0;  // chunk counter over the whole kernel
@@ -136,145 +126,91 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issue ===============================
-    const uint32_t idesc = umma_idesc_tf32(128, N);
-    long long c = 0;
-    int tl = 0;  // local tile counter
-    for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++tl) {
-      const int buf = tl & 1;
-      if (lane == 0) mbar_wait(bar_acc_empty + 8 * buf, (uint32_t)(((tl >> 1) & 1) ^ 1));
-      __syncwarp();
-      tc_fence_after();
-      const uint32_t dd = tmem_base + buf * N;
-      for (int kc = 0; kc < kc_total; ++kc, ++c) {
-        const int s = (int)(c % NSTG);
-        if (lane == 0) mbar_wait(bar_full + 8 * s, (uint32_t)((c / NSTG) & 1));
-        __syncwarp();
-        tc_fence_after();
-        const uint64_t da = umma_desc(sbase + s * STG_BYTES);
-        const uint64_t db = umma_desc(sbase + s * STG_BYTES + A_BYTES);
-        if (elect_one()) {
+    return;
+  }
+  // ================= consumers: wgmma (64 rows x N per warp group), then the epilogue from registers =================
+  // accumulator fragment of m64nNk8: acc[4j + 2i + e] is row 16 * (warp & 3) + lane / 4 + 8 i, column 8j + 2 (lane & 3) + e
+  const int half = wg - 1;
+  const int rq = 64 * half + 16 * (warp & 3) + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  long long c = 0;
+  for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
+    const int b = (int)(w / p.n_tiles), tile = (int)(w - (long long)b * p.n_tiles);
+    float acc[N / 2];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_tf32(dd, da + 2 * k, db + 2 * k, idesc, (uint32_t)((kc | k) != 0));
-          umma_commit(bar_empty + 8 * s);
-          if (kc == kc_total - 1) umma_commit(bar_acc_full + 8 * buf);
-        }
-        __syncwarp();
-      }
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    for (int kc = 0; kc < kc_total; ++kc, ++c) {
+      const int s = (int)(c % NSTG);
+      mbar_wait(bar_full + 8 * s, (uint32_t)((c / NSTG) & 1));
+      const uint64_t da = gmma_desc(sbase + s * STG_BYTES + half * (A_BYTES / 2));
+      const uint64_t db = gmma_desc(sbase + s * STG_BYTES + A_BYTES);
+      wgmma_fence(acc, N / 2);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) Wgmma<N>::mma(acc, da + 2 * k, db + 2 * k, (uint32_t)((kc | k) != 0));
+      wgmma_commit();
+      wgmma_wait0(acc, N / 2);
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
     }
-  } else {
-    // =============================== epilogue (thread = row) ===============================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;
-    const uint32_t t_lane = ((uint32_t)(q * 32)) << 16;
-    int tl = 0;
-    for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++tl) {
-      const int b = (int)(w / p.n_tiles), tile = (int)(w - (long long)b * p.n_tiles);
-      const int buf = tl & 1;
-      const long long r = (long long)tile * 128 + row;
-      const bool valid = r < p.n_rows;
-      // row bases of the optional epilogue operands (loads issued before the accumulator wait)
-      const float* a0 = nullptr;
-      const float* a1 = nullptr;
-      const float* pp = nullptr;
-      const float* rr = nullptr;
-      if (valid) {
-        if (p.add[0]) a0 = p.add[0] + (long long)b * p.add_bs[0] + (long long)(p.add_idx[0] ? __ldg(p.add_idx[0] + r) : r) * N;
-        if (p.add[1]) a1 = p.add[1] + (long long)b * p.add_bs[1] + (long long)(p.add_idx[1] ? __ldg(p.add_idx[1] + r) : r) * N;
-        if (p.post) pp = p.post + (long long)b * p.post_bs + (long long)(p.post_idx ? __ldg(p.post_idx + r) : r) * N;
-        if (p.res) rr = p.res + (long long)b * p.res_bs + r * N;
-      }
-      if (lane == 0) mbar_wait(bar_acc_full + 8 * buf, (uint32_t)((tl >> 1) & 1));
-      __syncwarp();
-      tc_fence_after();
-      const uint32_t acc = tmem_base + buf * N + t_lane;
-      float mu = 0.f, rstd = 1.f;
-      if (p.gamma) {  // LayerNorm statistics: first pass over the accumulator row
-        float sm = 0.f, sq = 0.f;
-        for (int c = 0; c < N / 32; ++c) {
-          float v[32];
-          tmem_ld32(acc + 32 * c, v);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float x = v[i] + sprm[32 * c + i];
-            sm += x;
-            sq = fmaf(x, x, sq);
-          }
+    for (int i = 0; i < 2; ++i) {
+      const long long r = (long long)tile * 128 + rq + 8 * i;
+      const bool valid = r < p.n_rows;
+      float v[N / 4];
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) {
+        v[2 * j] = acc[4 * j + 2 * i] + sprm[8 * j + cq];
+        v[2 * j + 1] = acc[4 * j + 2 * i + 1] + sprm[8 * j + cq + 1];
+      }
+      float mu = 0.f, rstd = 1.f;
+      if (p.gamma) {  // LayerNorm statistics of the row: this thread's N / 4 columns, then the 4 threads of the quad
+        float sm = 0.f, sq = 0.f;
+#pragma unroll
+        for (int j = 0; j < N / 4; ++j) {
+          sm += v[j];
+          sq = fmaf(v[j], v[j], sq);
         }
+        sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+        sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+        sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+        sq += __shfl_xor_sync(0xffffffffu, sq, 2);
         mu = sm * (1.0f / N);
         rstd = rsqrtf(fmaxf(sq * (1.0f / N) - mu * mu, 0.f) + p.eps);
       }
+      if (!valid) continue;
+      for (int a = 0; a < 2; ++a)
+        if (p.add[a])
+          add_row2(v, p.add[a] + (long long)b * p.add_bs[a] + (long long)(p.add_idx[a] ? __ldg(p.add_idx[a] + r) : r) * N + cq, N);
+      if (p.act) {
+#pragma unroll
+        for (int j = 0; j < N / 4; ++j) v[j] = silu_fast(v[j]);
+      }
+      if (p.gamma) {
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+          v[2 * j] = fmaf((v[2 * j] - mu) * rstd, sprm[N + 8 * j + cq], sprm[2 * N + 8 * j + cq]);
+          v[2 * j + 1] = fmaf((v[2 * j + 1] - mu) * rstd, sprm[N + 8 * j + cq + 1], sprm[2 * N + 8 * j + cq + 1]);
+        }
+      }
+      if (p.post)
+        add_row2(v, p.post + (long long)b * p.post_bs + (long long)(p.post_idx ? __ldg(p.post_idx + r) : r) * N + cq, N);
+      if (p.out2) {
+        float* o2 = p.out2 + ((long long)b * p.n_rows + r) * N + cq;
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) *reinterpret_cast<float2*>(o2 + 8 * j) = make_float2(v[2 * j], v[2 * j + 1]);
+      }
+      if (p.res) add_row2(v, p.res + (long long)b * p.res_bs + r * N + cq, N);
       float* orow = p.out + ((long long)b * p.n_rows + r) * p.n_real;
-      float* o2row = p.out2 ? p.out2 + ((long long)b * p.n_rows + r) * N : nullptr;
-      for (int c = 0; c < N / 32; ++c) {
-        float v[32];
-        tmem_ld32(acc + 32 * c, v);
-        if (c == N / 32 - 1) {  // the accumulator buffer is in registers: hand it back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(bar_acc_empty + 8 * buf);
-        }
-        if (!valid) continue;
+      if (p.n_real == N) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += sprm[32 * c + i];
-        if (a0) {
+        for (int j = 0; j < N / 8; ++j) *reinterpret_cast<float2*>(orow + 8 * j + cq) = make_float2(v[2 * j], v[2 * j + 1]);
+      } else {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 x = __ldg(reinterpret_cast<const float4*>(a0 + 32 * c) + i);
-            v[4 * i] += x.x; v[4 * i + 1] += x.y; v[4 * i + 2] += x.z; v[4 * i + 3] += x.w;
-          }
-        }
-        if (a1) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 x = __ldg(reinterpret_cast<const float4*>(a1 + 32 * c) + i);
-            v[4 * i] += x.x; v[4 * i + 1] += x.y; v[4 * i + 2] += x.z; v[4 * i + 3] += x.w;
-          }
-        }
-        if (p.act) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = silu_fast(v[i]);
-        }
-        if (p.gamma) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaf((v[i] - mu) * rstd, sprm[N + 32 * c + i], sprm[2 * N + 32 * c + i]);
-        }
-        if (pp) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 x = __ldg(reinterpret_cast<const float4*>(pp + 32 * c) + i);
-            v[4 * i] += x.x; v[4 * i + 1] += x.y; v[4 * i + 2] += x.z; v[4 * i + 3] += x.w;
-          }
-        }
-        if (o2row) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            reinterpret_cast<float4*>(o2row + 32 * c)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-        }
-        if (rr) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 x = __ldg(reinterpret_cast<const float4*>(rr + 32 * c) + i);
-            v[4 * i] += x.x; v[4 * i + 1] += x.y; v[4 * i + 2] += x.z; v[4 * i + 3] += x.w;
-          }
-        }
-        if (p.n_real == N) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            reinterpret_cast<float4*>(orow + 32 * c)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * c + i < p.n_real) orow[32 * c + i] = v[i];
+        for (int j = 0; j < N / 8; ++j) {
+          if (8 * j + cq < p.n_real) orow[8 * j + cq] = v[2 * j];
+          if (8 * j + cq + 1 < p.n_real) orow[8 * j + cq + 1] = v[2 * j + 1];
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TM_COLS) : "memory");
   }
 }
 
@@ -502,7 +438,7 @@ int tc_mlp2_packed(const NlamMlp* m, const NlamRowSrc* srcs, int n_src, const Nl
   const long long total = (long long)B * n_rows * kp;
   {
     ProfScope ps("pack_rows_kernel", st, 4.0 * total + 4.0 * (double)B * n_rows * m->in_dim);
-    pack_rows_kernel<<<(int)std::min<long long>((total + 255) / 256, 148 * 16), 256, 0, st>>>(
+    pack_rows_kernel<<<(int)std::min<long long>((total + 255) / 256, 132 * 16), 256, 0, st>>>(
         sp[0], sp[1], sp[2], sp[3], d[0], d[1], d[2], d[3], bs[0], bs[1], bs[2], bs[3], packed, kp, n_rows, B, ix);
   }
   count_launch();
@@ -538,7 +474,7 @@ extern "C" int nlam_pack_rows(const float* s0, const float* s1, const float* s2,
   if (total == 0) return NLAM_OK;
   {
     nlam::ProfScope ps("pack_rows_kernel", st, 8.0 * total);
-    nlam::pack_rows_kernel<<<(int)std::min<long long>((total + 255) / 256, 148 * 16), 256, 0, st>>>(
+    nlam::pack_rows_kernel<<<(int)std::min<long long>((total + 255) / 256, 132 * 16), 256, 0, st>>>(
         s0, s1, s2, s3, d0, d1, d2, d3, bs0, bs1, bs2, bs3, out, kp, n_rows, B, nlam::PackIdx{{nullptr, nullptr, nullptr, nullptr}});
   }
   nlam::count_launch();

@@ -1,5 +1,5 @@
-// Shared device-side PTX wrappers (mbarrier, TMA, tcgen05/TMEM, cp.async) and host-side tensor-map
-// helpers for the sm_100a tensor-core kernels (tc.cu, tc2.cu).
+// Shared device-side PTX wrappers (mbarrier, TMA, wgmma, cp.async) and host-side tensor-map helpers for the sm_90a
+// tensor-core kernels.
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -53,7 +53,7 @@ __device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
       : "memory");
   return done != 0;
 }
-// one elected lane of a converged warp (the warp stays in uniform control flow, so tcgen05.mma / TMA operands live in
+// one elected lane of a converged warp (the warp stays in uniform control flow, so TMA operands live in
 // uniform registers instead of going through an R2UR + waterfall loop per instruction)
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -71,8 +71,6 @@ __device__ __forceinline__ bool mbar_test_u(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int n) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
@@ -91,7 +89,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 // L2 eviction policies: the streamed edge tiles (hundreds of MB per layer at the bench batch) must
-// not push the small, heavily re-read node rows (gather sources) out of the 126 MB L2.
+// not push the small, heavily re-read node rows (gather sources) out of the 50 MB L2.
 __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -113,15 +111,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
       " [%0], [%1, {%3, %4, %5}], [%2], %6;"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(pol)
-      : "memory");
-}
-// TMA tile::gather4: 4 rows (arbitrary row indices) x 32 columns -> 4 consecutive 128-byte smem rows
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap* map, uint32_t bar, int col, int r0, int r1,
-                                            int r2, int r3, uint64_t pol) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2], %8;"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "l"(pol)
       : "memory");
 }
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
@@ -165,158 +154,27 @@ __device__ __forceinline__ void cp_async_wait_all() {
   asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
 }
 
-// UMMA shared-memory descriptor: K-major, 128-byte swizzle, 8-row groups 1024 B apart
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-//  layout_type [61,64) with SWIZZLE_128B = 2).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
+// wgmma shared-memory matrix descriptor (sm_90): K-major, 128-byte swizzle, 8-row groups 1024 B apart
+// (start >> 4 at [0,14), LBO >> 4 at [16,30) (unused for swizzled K-major), SBO >> 4 at [32,46), layout [62,64): 1 = SWIZZLE_128B).
+// Advancing K by 8 tf32 elements inside the 128-byte swizzle row adds 32 B (= 2 in the start field).
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;                // LBO (ignored for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;      // SBO
-  d |= (uint64_t)1 << 46;                // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// instruction descriptor, kind::tf32: D=f32 (bits 4-5 = 1), A=B=tf32 (bits 7-9, 10-12 = 2),
-// both K-major, N>>3 at [17,23), M>>4 at [24,29)   (cute::UMMA::InstrDescriptor)
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// the accumulator registers are written asynchronously between wgmma issue and wgmma.wait_group: the empty asm statements
+// pin every read and write of them on the right side of the fence / wait
+__device__ __forceinline__ void wgmma_fence(float* acc, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (lane = row, column = k; 32-bit elements), B from shared memory
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n\t"
-      "tcgen05.wait::st.sync.aligned;"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n\t"
-      "tcgen05.wait::st.sync.aligned;"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, float a, float b) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};\n\t"
-      "tcgen05.wait::st.sync.aligned;"
-      ::"r"(taddr), "r"(__float_as_uint(a)), "r"(__float_as_uint(b))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// --- split issue / wait: a dependent TMEM access costs ~300 cycles; issue several, wait once.  The loaded registers
-// may only be read after tmem_ld_wait() AND a reg_fence32() on them (the compiler must not move their uses up).
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void reg_fence32(float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(""
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                 "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                 "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                 "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st32_nowait(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0(float* acc, int n) {
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(acc[i])::"memory");
 }
 
 // byte offset of 16-byte chunk `ch` (0..7) of row `row` inside a 128B-swizzled [128][32 float] block
@@ -338,29 +196,6 @@ __device__ __forceinline__ float4 lds128(const void* ptr) {
                : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
                : "r"(smem_u32(ptr)));
   return v;
-}
-// packed fp32 pairs (FADD2 / FMUL2 / FFMA2 on sm_100): one issue slot for two lanes of work
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  float2 d;
-  asm("add.rn.f32x2 %0, %1, %2;"
-      : "=l"(*reinterpret_cast<unsigned long long*>(&d))
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  float2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(*reinterpret_cast<unsigned long long*>(&d))
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return d;
-}
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(*reinterpret_cast<unsigned long long*>(&d))
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)),
-        "l"(*reinterpret_cast<unsigned long long*>(&c)));
-  return d;
 }
 __device__ __forceinline__ float tanh_fast(float x) {
   float t;
@@ -442,7 +277,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

@@ -16,16 +16,16 @@ from . import _lib, backward, ops
 from .networks import _aten_forward, make_mlp
 
 _DEFAULT_MATH = "auto"
-# in-place edge update of the middle layers of a no-grad stack (csrc/tc8.cu: TMA reduce-add of the message tiles); the
+# in-place edge update of the middle layers of a no-grad stack (csrc/fused.cu: each tile writes e + m over its own edge rows); the
 # library decides per call shape (nlam_inet_inplace_supported), other shapes stay out of place
 _INPLACE_EDGE_UPDATE = True
-# the node kernel of a stacked layer also computes the next layer's node projections (csrc/tc10.cu)
+# the node kernel of a stacked layer also computes the next layer's node projections (csrc/fused.cu)
 _CHAIN_PROJECTIONS = True
 _MATH_FLAGS = {"auto": 0, "tf32": _lib.MATH_TF32, "fp32": _lib.MATH_FP32}
 
 
 def set_default_math(mode):
-    """``"auto"`` (tcgen05 TF32 kernels where the shape is supported, exact fp32 kernels
+    """``"auto"`` (wgmma TF32 kernels where the shape is supported, exact fp32 kernels
     otherwise), ``"tf32"`` (require the tensor-core kernels) or ``"fp32"`` (exact FFMA)."""
     global _DEFAULT_MATH
     if mode not in _MATH_FLAGS:
@@ -81,7 +81,7 @@ def _aten_apply(mod, names, params, prefix, x):
 class InteractionNet(nn.Module):
     """Interaction network (Battaglia et al. 2016) message-passing layer:
     ``m_e = edge_mlp([e, x_sender, x_receiver])``; ``aggr_r = sum|mean_{e->r} m_e``;
-    ``rec' = rec + aggr_mlp([rec, aggr])``; ``e' = e + m`` — computed by fused sm_100a kernels.
+    ``rec' = rec + aggr_mlp([rec, aggr])``; ``e' = e + m`` — computed by fused sm_90a kernels.
     """
 
     propagation = False
@@ -194,7 +194,7 @@ class InteractionNet(nn.Module):
             if not t.is_cuda:
                 raise RuntimeError(
                     f"neural_lam_b200.{type(self).__name__}: {name} is on {t.device}; this layer runs on "
-                    "CUDA (B200) tensors only — there is no CPU fallback")
+                    "CUDA tensors only — there is no CPU fallback")
             if t.dtype != torch.float32:
                 raise TypeError(f"{name}: float32 expected, got {t.dtype}")
             if t.dim() not in (2, 3) or t.shape[-1] != self.input_dim:
@@ -220,7 +220,7 @@ class InteractionNet(nn.Module):
     def _kernel_messages(self, send, rec, edge):
         """Messages in ORIGINAL edge order + aggregate, composed from the row-MLP and
         segment-sum kernels (used for SplitMLPs layers and ``propagate``)."""
-        fl = self._math_only_flags()  # SplitMLPs chunks: gather-pack + the generic tcgen05 Linear kernel (or exact fp32)
+        fl = self._math_only_flags()  # SplitMLPs chunks: gather-pack + the generic wgmma Linear kernel (or exact fp32)
         idx = [None, self._src32, self._dst32]
         outs = []
         for m, r0, r1 in _mlp_chunks(self.edge_mlp, self.num_edges):
@@ -346,7 +346,7 @@ class InteractionNet(nn.Module):
         tensor belongs to the caller — e.g. the cached static embedding — and is never written).  Same values as
         ``forward``.  ``proj_in``: this layer's node projections, computed by the previous layer's node kernel;
         ``next_layer``: the following layer of the stack — when the library supports it for both, this call's node kernel
-        also computes that layer's projections (csrc/tc10.cu).  Returns ``(node_rep', edge_rep' | None, proj_next | None)``."""
+        also computes that layer's projections (csrc/fused.cu).  Returns ``(node_rep', edge_rep' | None, proj_next | None)``."""
         if self._halo is not None or not (self.update_edges and self._fusable() and self._is_sorted):
             assert proj_in is None
             return (*self.forward(node_rep, node_rep, edge_rep), None)

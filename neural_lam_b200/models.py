@@ -1,5 +1,5 @@
 """Graph step predictors (GraphLAM / HiLAM) and the autoregressive forecaster with the
-reference's structure, parameter names and forward semantics, running on the B200 kernels.
+reference's structure, parameter names and forward semantics, running on the sm_90a kernels.
 
 Reference files mirrored (neural_lam/models/...):
   step_predictors/base.py        StepPredictor: expand_to_batch :122-139, clamped update :335-396

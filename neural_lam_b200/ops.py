@@ -41,7 +41,7 @@ def _require_cuda(*tensors):
             continue
         if not t.is_cuda:
             raise RuntimeError(
-                "neural_lam_b200: tensors must live on a CUDA (B200) device — there is no CPU fallback "
+                "neural_lam_b200: tensors must live on a CUDA device — there is no CPU fallback "
                 "(got a tensor on %s)" % (t.device,)
             )
         if t.dtype != torch.float32:

@@ -8,7 +8,7 @@ It imports the reference's ``neural_lam/gnn_layers.py`` / ``utils/networks.py``
 unmodified (``oracle/load_reference.py``), builds ``InteractionNet`` /
 ``PropagationNet`` instances exactly as the reference constructs them, runs
 forward + backward on seeded CPU fp32 inputs and stores inputs, weights, outputs
-and gradients as ``tests/golden/inet_cases.npz``.  The GPU box has no
+and gradients as ``tests/golden/inet_cases.*.npz``.  The GPU box has no
 ``/root/reference``; its tests compare against this file.
 """
 import os
@@ -18,8 +18,9 @@ import numpy as np
 import torch
 
 from . import load_reference
+from .shards import save_shards
 
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "inet_cases.npz")
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "inet_cases")
 
 
 def _rand_edge_index(n_send, n_rec, n_edges, seed=0):
@@ -106,8 +107,8 @@ def main():
         ).astype(str)
     blob["__names__"] = np.array(names)
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
-    np.savez_compressed(OUT, **blob)
-    print(f"wrote {OUT}: {len(names)} cases, {os.path.getsize(OUT)/1024:.1f} KiB")
+    paths = save_shards(OUT, blob)
+    print(f"wrote {len(paths)} files {OUT}.*.npz")
 
 
 if __name__ == "__main__":

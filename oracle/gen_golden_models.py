@@ -11,7 +11,7 @@ TEST INFRASTRUCTURE ONLY.  Run in the build container (needs /root/reference):
 format (``neural_lam_b200.synthetic.save_graph``), the reference model reads it with ITS OWN ``load_graph``, is
 initialised under ``torch.manual_seed``, and ``ARForecaster.forward`` is run on seeded CPU fp32 inputs.  Stored:
 the state_dict, the inputs, the rollout (and the predicted std where the model has one) ->
-``tests/golden/model_cases.npz``.  Both the CPU restatement (tests/test_oracle_models.py) and the CUDA path
+``tests/golden/model_cases.*.npz``.  Both the CPU restatement (tests/test_oracle_models.py) and the CUDA path
 (tests/test_models_golden.py, ``-m gpu``) are checked against this file.
 """
 import os
@@ -22,13 +22,14 @@ import numpy as np
 import torch
 
 from . import load_reference
+from .shards import save_shards
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "tests", "golden", "model_cases.npz")
+OUT = os.path.join(ROOT, "tests", "golden", "model_cases")
 
 # name -> (reference class, graph kwargs, datastore kwargs, model kwargs, B, T)
 CASES = {
-    # BASELINE config 2's model family (multiscale GraphLAM, H=64: the tcgen05 kernels) on a small grid
+    # BASELINE config 2's model family (multiscale GraphLAM, H=64: the fused tensor-core kernels) on a small grid
     "graph_lam_ms_h64": ("GraphLAM", dict(Nx=30, Ny=27, hierarchical=False),
                          dict(d_state=5, d_forcing=6, d_static=1, boundary_width=2),
                          dict(hidden_dim=64, processor_layers=2), 2, 3),
@@ -99,8 +100,8 @@ def main():
                 out[f"{name}/{k}"] = v
     out["__names__"] = np.array(list(CASES))
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
-    np.savez_compressed(OUT, **out)
-    print(f"wrote {OUT}: {len(CASES)} cases, {os.path.getsize(OUT) / 1e6:.2f} MB")
+    paths = save_shards(OUT, out)
+    print(f"wrote {len(paths)} files {OUT}.*.npz")
 
 
 if __name__ == "__main__":

@@ -1,17 +1,43 @@
-"""Loader for tests/golden/inet_cases.npz (generated from the reference source by
+"""Loader for tests/golden/inet_cases.*.npz (generated from the reference source by
 oracle/gen_golden.py)."""
 import ast
+import glob
 import os
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden", "inet_cases.npz")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "inet_cases")
+
+
+class Shards:
+    """The arrays of ``<stem>.<i>.npz`` (written by oracle/shards.py) as one mapping with an ``.files`` list."""
+
+    def __init__(self, stem):
+        paths = sorted(glob.glob(stem + ".*.npz"), key=lambda p: int(p.rsplit(".", 2)[1]))
+        if not paths:
+            raise FileNotFoundError(stem + ".*.npz")
+        self._src = {}
+        for path in paths:
+            z = np.load(path, allow_pickle=False)
+            for k in z.files:
+                self._src[k] = z
+        self.files = list(self._src)
+
+    def __getitem__(self, k):
+        return self._src[k][k]
+
+    def __contains__(self, k):
+        return k in self._src
+
+
+def load_shards(stem):
+    return Shards(stem)
 
 
 class GoldenCase:
-    """One case of tests/golden/inet_cases.npz (generated from the reference source
+    """One case of tests/golden/inet_cases.*.npz (generated from the reference source
     by oracle/gen_golden.py)."""
 
     def __init__(self, blob, name):
@@ -43,5 +69,5 @@ class GoldenCase:
 
 
 def load_golden_cases():
-    blob = np.load(GOLDEN, allow_pickle=False)
+    blob = load_shards(GOLDEN)
     return [GoldenCase(blob, str(n)) for n in blob["__names__"]]

@@ -1,4 +1,4 @@
-"""Loader for tests/golden/model_cases.npz (generated from the reference's own model source by
+"""Loader for tests/golden/model_cases.*.npz (generated from the reference's own model source by
 oracle/gen_golden_models.py) + builders of the product model / oracle inputs for a case."""
 import ast
 import os
@@ -6,8 +6,10 @@ import os
 import numpy as np
 import torch
 
+from golden_util import load_shards
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden", "model_cases.npz")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "model_cases")
 
 KIND = {"GraphLAM": "graph_lam", "HiLAM": "hi_lam", "HiLAMParallel": "hi_lam_parallel"}
 
@@ -61,5 +63,5 @@ class ModelCase:
 
 
 def load_model_cases():
-    blob = np.load(GOLDEN, allow_pickle=False)
+    blob = load_shards(GOLDEN)
     return [ModelCase(blob, str(n)) for n in blob["__names__"]]

@@ -28,7 +28,7 @@ def test_library_loads_and_exports_every_declared_symbol():
         assert n in _lib.SYMBOLS, f"{n} has no ctypes prototype"
     assert set(_lib.SYMBOLS) == set(names)
     assert _lib.lib().nlam_abi_version() == 1
-    assert b"sm_100a" in _lib.lib().nlam_build_info()
+    assert b"sm_90a" in _lib.lib().nlam_build_info()
 
 
 def test_struct_layout_matches_header():

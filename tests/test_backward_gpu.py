@@ -1,4 +1,4 @@
-"""The hand-written backward (neural_lam_b200/backward.py: generic tcgen05 Linear for dX / split-K dW, SiLU / LayerNorm
+"""The hand-written backward (neural_lam_b200/backward.py: generic wgmma Linear for dX / split-K dW, SiLU / LayerNorm
 backward, CSR segment sums) against (1) the gradients of the reference's own source stored in
 tests/golden/inet_cases.npz (H = 64 cases), (2) autograd through the fp64 oracle on fresh graphs — all inputs and all
 parameters — and (3) a whole GraphLAM training step; plus the proof that no cuBLAS / ATen GEMM runs in it.

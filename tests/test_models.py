@@ -151,7 +151,7 @@ def test_training_step_gradients_match_oracle():
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,hidden", [("hi_lam", 128), ("graph_lam_multiscale", 256)])
 def test_wide_hidden_models_run_on_the_generic_tensor_core_path(kind, hidden):
-    """BASELINE configs 3-5 use hidden_dim 128 / 256: every per-step launch is the generic tcgen05 Linear kernel (tc7.cu)
+    """BASELINE configs 3-5 use hidden_dim 128 / 256: every per-step launch is the generic wgmma Linear kernel (tc7.cu)
     or an index kernel — no FFMA row-MLP — and the rollout matches the fp64 oracle within the TF32 bound
     (|err| <= max(3 x the reference's TF32 configuration, 1e-2), as in tests/test_real_size.py)."""
     from neural_lam_b200 import ops

@@ -1,16 +1,16 @@
 """Model-level oracle pinning (SURVEY.md 8 rows a10-a16): the CPU restatement
 ``oracle/reference_port.graph_model_forward`` / ``ar_rollout`` against golden vectors produced by the reference's
 OWN ``graph/base.py`` + ``graph_lam.py`` + ``hierarchical.py`` + ``hi_lam.py`` + ``hi_lam_parallel.py`` +
-``forecasters/autoregressive.py`` (``oracle/gen_golden_models.py``), and — where /root/reference is present —
-against the reference classes run live."""
+``forecasters/autoregressive.py`` (``oracle/gen_golden_models.py``), and the graph loader / generator against the
+reference's results stored by ``oracle/gen_golden_refchecks.py``."""
 import os
 import tempfile
 
 import pytest
 import torch
 
+from golden_util import load_shards
 from model_golden_util import load_model_cases
-from oracle import load_reference
 from oracle import reference_port as rp
 
 CASES = load_model_cases()
@@ -41,45 +41,42 @@ def test_state_dict_names_match_reference():
         assert set(model.state_dict()) == set(case.params), case.name
 
 
-@pytest.mark.skipif(not load_reference.available(), reason="needs /root/reference (build container only)")
-def test_golden_file_reproduces_from_reference_source():
-    """Re-run the reference classes for the smallest case and compare with the committed file."""
-    from oracle import gen_golden_models as gg
-
-    ref = load_reference.load_models()
-    with tempfile.TemporaryDirectory() as tmp:
-        blob = gg.run_case(ref, "graph_lam_opts_h16", tmp)
-    case = next(c for c in CASES if c.name == "graph_lam_opts_h16")
-    torch.testing.assert_close(torch.from_numpy(blob["pred"]), case.pred, rtol=1e-6, atol=1e-6)
-    torch.testing.assert_close(torch.from_numpy(blob["pred_std"]), case.pred_std, rtol=1e-6, atol=1e-6)
+REFCHECKS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_checks")
 
 
-@pytest.mark.skipif(not load_reference.available(), reason="needs /root/reference (build container only)")
+def _stored(blob, pre):
+    """one tensor, or the per-level list stored as <pre>/0, <pre>/1, ..."""
+    if pre in blob:
+        return torch.from_numpy(blob[pre])
+    out = []
+    while f"{pre}/{len(out)}" in blob:
+        out.append(torch.from_numpy(blob[f"{pre}/{len(out)}"]))
+    return out
+
+
 def test_reference_load_graph_reads_generated_files():
-    """The reference's own ``load_graph`` accepts the directories ``synthetic.save_graph`` writes, and
-    ``synthetic.load_graph`` + ``normalize_graph`` arrive at the same tensors."""
+    """``synthetic.load_graph`` + ``normalize_graph`` on the directories ``synthetic.save_graph`` writes arrive at the
+    tensors the reference's own ``load_graph`` read from the same directories (stored in
+    tests/golden/reference_checks.*.npz by oracle/gen_golden_refchecks.py)."""
     from neural_lam_b200 import synthetic
 
-    ref = load_reference.load_models()
+    blob = load_shards(REFCHECKS)
     for hier in (False, True):
         spec = synthetic.make_graph_spec(30, 27, hierarchical=hier)
         with tempfile.TemporaryDirectory() as tmp:
             synthetic.save_graph(spec, tmp)
-            span = float(max(spec["grid_xy"][:, 0].max() - spec["grid_xy"][:, 0].min(),
-                             spec["grid_xy"][:, 1].max() - spec["grid_xy"][:, 1].min()))
-            is_hier, g = ref.load_graph(tmp, mesh_node_features_scaling=span)
             ours = synthetic.normalize_graph(synthetic.load_graph(tmp, spec["grid_xy"]))
-        assert is_hier == hier
+        g = lambda k: _stored(blob, f"load_graph/{int(hier)}/{k}")  # noqa: E731
         for k in ("g2m_features", "m2g_features", "g2m_edge_index", "m2g_edge_index"):
-            torch.testing.assert_close(ours[k], g[k], rtol=0, atol=0)
+            torch.testing.assert_close(ours[k], g(k), rtol=0, atol=0)
         for k in ("m2m_features", "m2m_edge_index", "mesh_static_features", "mesh_up_features", "mesh_down_edge_index"):
-            a, b = ours[k], g[k]
             if hier:
-                assert len(a) == len(b)
+                a, b = ours[k], g(k)
+                assert len(a) == len(b) > 0
                 for x, y in zip(a, b):
                     torch.testing.assert_close(x, y, rtol=0, atol=0)
             elif k in ("m2m_features", "m2m_edge_index", "mesh_static_features"):
-                torch.testing.assert_close(a, b, rtol=0, atol=0)
+                torch.testing.assert_close(ours[k], g(k), rtol=0, atol=0)
 
 
 def test_legacy_graph_directory_is_zero_indexed(tmp_path):
@@ -108,19 +105,19 @@ def _edge_set(ei, feat):
     return sorted((int(a), int(b)) + tuple(round(float(x), 4) for x in f) for a, b, f in zip(ei[0], ei[1], feat))
 
 
-@pytest.mark.skipif(not load_reference.available(), reason="needs /root/reference (build container only)")
 @pytest.mark.parametrize("hier", [False, True])
 def test_graph_generator_matches_reference_create_graph(hier):
     """``synthetic.make_graph_spec`` (vectorised) against the reference's own ``create_graph`` (networkx loops,
-    create_graph.py:356-862, run unmodified through oracle/load_create_graph.py) on a NON-square grid: identical edge
-    sets and edge features for g2m (radius 0.67 x the mesh spacing along the first axis), m2g (4 nearest), every m2m
-    level, the up / down edges, and identical mesh node positions."""
+    create_graph.py:356-862, run unmodified through oracle/load_create_graph.py; its graphs are stored in
+    tests/golden/reference_checks.*.npz) on a NON-square grid: identical edge sets and edge features for g2m (radius
+    0.67 x the mesh spacing along the first axis), m2g (4 nearest), every m2m level, the up / down edges, and identical
+    mesh node positions."""
     from neural_lam_b200 import synthetic
-    from oracle import load_create_graph as lcg
 
-    if not lcg.available():
-        pytest.skip("networkx / reference create_graph not available")
-    ref = lcg.reference_create_graph(30, 27, hierarchical=hier)
+    blob = load_shards(REFCHECKS)
+    ref = {k: _stored(blob, f"create_graph/{int(hier)}/{k}") for k in (
+        "g2m_edge_index", "g2m_features", "m2g_edge_index", "m2g_features", "m2m_edge_index", "m2m_features", "mesh_features",
+        "mesh_up_edge_index", "mesh_up_features", "mesh_down_edge_index", "mesh_down_features")}
     mine = synthetic.make_graph_spec(30, 27, hierarchical=hier)
     for k in ("g2m", "m2g"):
         assert _edge_set(ref[f"{k}_edge_index"], ref[f"{k}_features"]) == _edge_set(mine[f"{k}_edge_index"], mine[f"{k}_features"]), k
@@ -136,30 +133,3 @@ def test_graph_generator_matches_reference_create_graph(hier):
             for l in range(len(mine[f"{k}_edge_index"])):
                 assert _edge_set(ref[f"{k}_edge_index"][l], ref[f"{k}_features"][l]) == \
                     _edge_set(mine[f"{k}_edge_index"][l], mine[f"{k}_features"][l]), f"{k} level {l}"
-
-
-@pytest.mark.skipif(not load_reference.available(), reason="needs /root/reference (build container only)")
-@pytest.mark.parametrize("hier", [False, True])
-def test_saved_graphs_pass_the_reference_validator(hier, tmp_path):
-    """``synthetic.save_graph`` output through the reference's stand-alone on-disk validator docs/validate_graph.py."""
-    import importlib.util
-    import sys
-
-    from neural_lam_b200 import synthetic
-
-    path = os.path.join(load_reference.REFERENCE_ROOT, "docs", "validate_graph.py")
-    spec = importlib.util.spec_from_file_location("_ref_validate_graph", path)
-    vg = importlib.util.module_from_spec(spec)
-    sys.modules["_ref_validate_graph"] = vg
-    spec.loader.exec_module(vg)
-    g = synthetic.make_graph_spec(30, 27, hierarchical=hier)
-    synthetic.save_graph(g, str(tmp_path))
-    synthetic.save_graph_csr_cache(str(tmp_path))     # the extra <set>_csr.pt files must not disturb the validator
-    import warnings
-
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        report, _, props = vg.validate_graph_directory(str(tmp_path))
-    assert report.ok, [r for r in report.results if getattr(r, "status", "PASS") != "PASS"]
-    assert props.is_hierarchical == hier and props.num_grid_nodes == 810
-    assert props.num_mesh_nodes_per_level == ([81, 9] if hier else [81])

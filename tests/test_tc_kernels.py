@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 (TF32 tensor-core) kernels, through the C ABI, against the CPU oracle.
+"""Parity of the wgmma (TF32 tensor-core) kernels, through the C ABI, against the CPU oracle.
 
 Stated tolerance (TF32 inputs, fp32 accumulate; LayerNorm outputs are O(1)):
   * |kernel - fp64 oracle| <= 1e-2 absolute per InteractionNet call, and
@@ -53,7 +53,7 @@ CASES = [
     ("empty_receivers", 40, 600, 300, 2, True, "sum", False, True, False),
     ("single_tile", 5, 4, 10, 1, True, "sum", False, True, False),
     ("deg128", 300, 3, 300, 2, False, "sum", False, True, False),
-    # batch-broadcast edge features, no edge update, large sender set -> tc_edge_bcast_kernel (tc6.cu)
+    # batch-broadcast edge features, no edge update, large sender set -> tc_edge_bcast_kernel
     ("bcast_g2m", 3000, 200, 2500, 3, False, "sum", False, True, True),
     ("bcast_mean_b1", 3000, 200, 2500, 1, False, "mean", False, True, True),
     ("bcast_many_items", 60000, 3000, 40000, 5, False, "sum", False, True, True),
@@ -119,7 +119,7 @@ GEN_CASES = [
 
 @pytest.mark.parametrize("case", GEN_CASES, ids=[c[0] for c in GEN_CASES])
 def test_generic_tensor_core_path_vs_oracle(case):
-    """H = 128 / 256 (BASELINE configs 3-5) and PropagationNet: the generic tcgen05 Linear kernel (tc7.cu) — node
+    """H = 128 / 256 (BASELINE configs 3-5) and PropagationNet: the generic wgmma Linear kernel (tc7.cu) — node
     projections, two edge layers, CSR segment sum, two node layers — against the fp64 oracle, same bound as above."""
     name, cls, H, ns, nr, ne, B, upd, aggr, expand = case
     ei = _graph(ns, nr, ne, 3, True)
@@ -200,7 +200,7 @@ def test_tf32_requested_but_unsupported_raises_and_auto_falls_back():
         r_o, e_o = rp.interaction_net({k: v.cpu() for k, v in net_auto.state_dict().items()}, ei, *[t.cpu() for t in x])
         torch.testing.assert_close(r.cpu(), r_o, rtol=2e-5, atol=2e-5)  # exact-fp32 kernels were used
         net_tf = nlb.InteractionNet(ei, H, math="tf32").to(DEV)
-        with pytest.raises(_lib.NlamError, match="not supported by the tcgen05"):
+        with pytest.raises(_lib.NlamError, match="not supported by the tensor-core"):
             net_tf(*x)
 
 
@@ -213,7 +213,7 @@ ROW_CASES = [
     ("output_map_17", [64, 64, 17], [(2, 500, 64)], None, False),
     ("grid_embedder_56", [56, 64, 64], [(2, 400, 17), (2, 400, 17), (2, 400, 18), (400, 4)], None, True),
     ("one_row", [64, 64, 64], [(1, 1, 64)], None, True),
-    # streaming kernel (tc4.cu), several tiles per CTA, partial last tile
+    # row kernel, several tiles per CTA, partial last tile
     ("enc_many_tiles", [64, 64, 64], [(2, 128 * 300 + 77, 64)], 0, True),
     ("node_many_tiles", [128, 64, 64], [(2, 128 * 200 + 3, 64), (2, 128 * 200 + 3, 64)], 0, True),
     ("node_res_aggr_many", [128, 64, 64], [(2, 128 * 160 + 9, 64), (2, 128 * 160 + 9, 64)], 1, True),
@@ -223,6 +223,8 @@ ROW_CASES = [
     ("embedder_rows_not_mult4", [56, 64, 64], [(2, 401, 17), (2, 401, 17), (2, 401, 18), (401, 4)], None, True),
     ("output_map_many_tiles", [64, 64, 17], [(3, 128 * 200 + 5, 64)], None, False),
     ("narrow_in_narrow_out", [20, 64, 9], [(2, 1000, 13), (2, 1000, 7)], None, False),
+    # a source whose width is a multiple of 4 starting at a column that is not (grid embedder, d_state 5, d_forcing 12)
+    ("embedder_unaligned_offset", [24, 64, 64], [(2, 700, 5), (2, 700, 5), (2, 700, 12), (700, 2)], None, True),
 ]
 
 
@@ -300,7 +302,7 @@ def test_model_rollout_tf32_vs_oracle(kind):
 
 
 def test_split_edge_kernel_v2_matches_v1_and_oracle():
-    """Both formulations of the first edge Linear — split (node projections + tc5.cu, NLAM_TC_EDGE=v2) and K=192 with
+    """Both formulations of the first edge Linear — split (node projections + K=64 edge kernel, NLAM_TC_EDGE=v2) and K=192 with
     raw gathered rows (tc.cu, NLAM_TC_EDGE=v1); forced in a fresh process, the selection is read once per process —
     against the fp64 oracle."""
     import os
@@ -370,7 +372,7 @@ ELL_CASES = [
 
 @pytest.mark.parametrize("case", ELL_CASES, ids=[c[0] for c in ELL_CASES])
 def test_uniform_degree_edge_kernels_vs_oracle(case):
-    """Uniform in-degree edge sets with update_edges=False take the receiver-tiled kernels of tc3.cu."""
+    """Uniform in-degree edge sets with update_edges=False take the uniform-degree edge path (tc_ell_window_kernel)."""
     name, ns, nr, d, B, aggr, expand, bcast = case
     ei = _ell_graph(ns, nr, d, 1)
     torch.manual_seed(0)
@@ -450,8 +452,8 @@ RMW_CASES = [
 
 @pytest.mark.parametrize("case", RMW_CASES, ids=[c[0] for c in RMW_CASES])
 def test_inplace_edge_update_kernel(case):
-    """tc8.cu: e += m as a TMA reduce-add of the staged message tiles (edge_out aliases edge) and the no-edge-output
-    mode, against the out-of-place kernel (tc5.cu) on the same inputs and against the fp64 oracle."""
+    """tc_edge_rmw_kernel: e += m written over the edge tensor (edge_out aliases edge) and the no-edge-output
+    mode, against the out-of-place kernel (tc_edge3_kernel) on the same inputs and against the fp64 oracle."""
     name, nn_, ne, B = case
     ei = _graph(nn_, nn_, ne, 3, True)
     if name == "empty_receivers":  # two thirds of the nodes receive nothing
@@ -519,7 +521,7 @@ def test_stack_updates_private_edge_tensor_in_place():
             got, e_none = seq(x, e_in, keep_edge_rep=False)
     assert e_none is None
     assert prof.names().count("tc_edge_rmw_kernel") == 3 and prof.names().count("tc_edge3_kernel") == 1, prof.names()
-    # the node kernel of layers 1-3 also computes the next layer's node projections (tc10.cu): one projection launch (layer 1)
+    # the node kernel of layers 1-3 also computes the next layer's node projections: one projection launch (layer 1)
     # and one plain node update (layer 4) remain
     assert prof.names().count("tc_node_proj_kernel") == 3 and prof.names().count("tc_rowlinear_kernel") == 1, prof.names()
     assert len(prof.names()) == 9, prof.names()
@@ -529,8 +531,8 @@ def test_stack_updates_private_edge_tensor_in_place():
 
 @pytest.mark.parametrize("with_boundary,B,G", [(True, 3, 1000), (False, 1, 128), (True, 2, 40 * 128 + 36)])
 def test_chained_node_update_output_map_step_epilogue(with_boundary, B, G):
-    """tc9.cu: node update of the mesh->grid layer + output_map + forecast-step epilogue in one launch, against the
-    two-kernel path (tc4.cu node update, then output_map + epilogue) on the same inputs: same TF32 products, same fp32
+    """tc_node_out_kernel: node update of the mesh->grid layer + output_map + forecast-step epilogue in one launch, against the
+    two-kernel path (row-kernel node update, then output_map + epilogue) on the same inputs: same TF32 products, same fp32
     formulas — the intermediate only stays in shared memory."""
     from neural_lam_b200.networks import make_mlp
     torch.manual_seed(3)
@@ -574,7 +576,7 @@ def test_chained_node_update_output_map_step_epilogue(with_boundary, B, G):
 @pytest.mark.parametrize("cls_name,H", [("InteractionNet", 64), ("PropagationNet", 64), ("InteractionNet", 128)])
 def test_split_mlps_layer_on_tensor_cores(cls_name, H):
     """SplitMLPs layers (reference gnn_layers.py:274-324; HiLAMParallel's per-level MLPs): every chunk's edge MLP runs as
-    gather-pack + two launches of the generic tcgen05 Linear kernel, the node MLPs on the row-MLP kernels — no SIMT math."""
+    gather-pack + two launches of the generic wgmma Linear kernel, the node MLPs on the row-MLP kernels — no SIMT math."""
     cls = getattr(nlb, cls_name)
     ns, nr, ne, B = 70, 50, 600, 2
     ei = _graph(ns, nr, ne, 4, False)  # chunks are defined on the layer's own (unsorted) edge order
@@ -597,7 +599,7 @@ def test_split_mlps_layer_on_tensor_cores(cls_name, H):
 
 @pytest.mark.parametrize("B,N", [(1, 100), (3, 500), (2, 128 * 3 + 5)])
 def test_node_kernel_with_next_layer_projections(B, N):
-    """tc10.cu through nlam_inet_fwd_chain: layer 1 produces the node projections of layer 2's edge MLP in its node kernel, layer
+    """tc_node_proj_kernel through nlam_inet_fwd_chain: layer 1 produces the node projections of layer 2's edge MLP in its node kernel, layer
     2 consumes them — against the unchained calls on the same inputs (same TF32 products: results agree to fp32 rounding)."""
     ei = _graph(N, N, 9 * N, 7, True)
     torch.manual_seed(4)
