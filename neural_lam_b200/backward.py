@@ -154,13 +154,23 @@ def grad_weight(gy, x, out, out_off=0, out_pitch=None, x_off=0, x_cols=None, x_p
 
 def grad_input(gy, w, n_in, w_off=0, ldw=None, res=None):
     """``gy · W[:, w_off : w_off + n_in]`` (+ res): gy (B, n, N) dense (N any width: zero-padded to a multiple of 32),
-    W (N, ldw) row-major."""
+    W (N, ldw) row-major.  n_in > 256 (wider than the Linear kernel's output): one Linear per 256-column block of W,
+    each written into its column slice of the result; ``res`` only with n_in <= 256."""
     B, n, N = gy.shape
     ldw = ldw if ldw is not None else w.shape[-1]
     Np = (N + 31) // 32 * 32
-    wT = transpose_pad(w, N, n_in, ldw, (N + 3) // 4 * 4, x_off=w_off)   # (n_in, N padded to a multiple of 4)
+    if res is not None and n_in > 256:
+        raise _lib.NlamError(f"grad_input: a residual needs n_in <= 256 (got {n_in})")
     x0 = gy if Np == N else pack([gy], Np)
-    return linear(x0, wT, n_in, ldw=wT.shape[1], w_cols=N, res=res)
+    out = None if n_in <= 256 else torch.empty((B, n, n_in), device=gy.device, dtype=torch.float32)
+    for c0 in range(0, n_in, 256):
+        kc = min(256, n_in - c0)
+        wT = transpose_pad(w, N, kc, ldw, (N + 3) // 4 * 4, x_off=w_off + c0)   # (kc, N padded to a multiple of 4)
+        part = linear(x0, wT, kc, ldw=wT.shape[1], w_cols=N, res=res)
+        if out is None:
+            return part
+        out[..., c0:c0 + kc] = part
+    return out
 
 
 def segment_sum(x, ptr, order, n_seg, mean=False):

@@ -506,13 +506,21 @@ static void grad_weight(Ctx& c, const float* gy, int64_t R, int N, const float* 
   c.a.release(m);
 }
 
-// out (B, n, n_in) = gy (B, n, N dense) · W[:, w_off .. w_off + n_in)  (+ res dense)
+// out (B, n, n_in) = gy (B, n, N dense) · W[:, w_off .. w_off + n_in)  (+ res dense).  The Linear kernel's output is at
+// most 256 wide: a wider n_in (an MLP input of more than 256 columns) runs one Linear per 256-column block of W into a
+// temporary that is copied into its column slice of out; res is only supported with n_in <= 256.
 static void grad_input(Ctx& c, const float* gy, int64_t n, int B, int N, const float* w, int ldw, int n_in, const float* res,
                        float* out) {
   const int Np = (N + 31) / 32 * 32, N4 = (N + 3) / 4 * 4;
+  const bool chunked = n_in > 256;
+  if (chunked && res) {
+    if (!c.a.dry && c.ok()) {
+      set_error("grad_input: a residual needs n_in <= 256 (got %d)", n_in);
+      c.rc = NLAM_E_UNSUPPORTED;
+    }
+    return;
+  }
   const size_t m = c.a.mark();
-  float* wT = c.a.get((size_t)n_in * N4);
-  transpose(c, w, N, N, n_in, ldw, wT, N4);
   const float* x0 = gy;
   if (Np != N) {
     float* pk = c.a.get((size_t)B * n * Np);
@@ -520,11 +528,23 @@ static void grad_input(Ctx& c, const float* gy, int64_t n, int B, int N, const f
       c.rc = nlam_pack_rows(gy, nullptr, nullptr, nullptr, N, 0, 0, 0, n * N, 0, 0, 0, pk, Np, n, B, c.st);
     x0 = pk;
   }
-  c.a.note();
-  LinArgs a;
-  a.x0 = x0; a.x0_bs = n * Np; a.k0 = Np; a.w = wT; a.ldw = N4; a.w_cols = N; a.n_out = n_in; a.res = res; a.res_bs = n * n_in;
-  a.n = n; a.B = B;
-  lin(c, a, out);
+  for (int c0 = 0; c0 < n_in; c0 += 256) {
+    const int kc = std::min(256, n_in - c0);
+    const size_t m2 = c.a.mark();
+    float* wT = c.a.get((size_t)kc * N4);
+    float* dst = chunked ? c.a.get((size_t)B * n * kc) : out;
+    c.a.note();
+    transpose(c, w + c0, N, N, kc, ldw, wT, N4);
+    LinArgs a;
+    a.x0 = x0; a.x0_bs = n * Np; a.k0 = Np; a.w = wT; a.ldw = N4; a.w_cols = N; a.n_out = kc; a.res = res; a.res_bs = n * kc;
+    a.n = n; a.B = B;
+    lin(c, a, dst);
+    if (chunked && !c.a.dry && c.ok() &&
+        cudaMemcpy2DAsync(out + c0, (size_t)n_in * 4, dst, (size_t)kc * 4, (size_t)kc * 4, (size_t)B * n, cudaMemcpyDeviceToDevice,
+                          c.st) != cudaSuccess)
+      c.rc = NLAM_E_CUDA;
+    c.a.release(m2);
+  }
   c.a.release(m);
 }
 
