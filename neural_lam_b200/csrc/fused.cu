@@ -99,15 +99,6 @@ struct FzParams {
   int n_tiles1, B1;
 };
 
-// operands are rounded to TF32 (round to nearest) when written to shared memory; the MMA would otherwise drop the low
-// mantissa bits (a bias toward zero)
-__device__ __forceinline__ float tf32r(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
-__device__ __forceinline__ float4 tf32r4(float4 v) { return make_float4(tf32r(v.x), tf32r(v.y), tf32r(v.z), tf32r(v.w)); }
-
 // byte offset of operand element (row R, column c) in a 128B-swizzled operand stored as 32-column chunks
 __device__ __forceinline__ uint32_t fz_off(uint32_t chunk_bytes, int R, int c) {
   return (uint32_t)(c >> 5) * chunk_bytes + swz(R, (c & 31) >> 2) + (uint32_t)(c & 3) * 4;

@@ -7,7 +7,9 @@
 //
 // One CTA tile = 128 rows x N (N = the full output width <= 256), K streamed in 32-column chunks through a ring of
 // shared-memory stages: the X chunk (16 KB) and the W chunk (N x 128 B, L2 resident) arrive by TMA with 128-byte swizzle,
-// and two consumer warp groups each run `wgmma.mma_async m64nNk8 .tf32` on their 64 rows of the stage, accumulating in
+// the two consumer warp groups round the stage to TF32 in place (to nearest, as fused.cu does: TMA copies raw fp32, which
+// the MMA would truncate; each warp group rounds its 64 rows of X and half of the W chunk, then fence.proxy.async and a
+// named barrier of both), and each runs `wgmma.mma_async m64nNk8 .tf32` on its 64 rows of the stage, accumulating in
 // registers; the epilogue works on the accumulator fragments (a row is spread over the 4 threads of a quad; LayerNorm
 // statistics are reduced with two shuffles).  Warp group 0 is the TMA producer.
 // An MLP (reference utils/networks.py:27-40) is two launches with the hidden activations in a workspace; an
@@ -131,6 +133,7 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   // ================= consumers: wgmma (64 rows x N per warp group), then the epilogue from registers =================
   // accumulator fragment of m64nNk8: acc[4j + 2i + e] is row 16 * (warp & 3) + lane / 4 + 8 i, column 8j + 2 (lane & 3) + e
   const int half = wg - 1;
+  const int ct = tid - 128, ct128 = tid & 127;  // thread index among the 256 consumer threads / in its warp group
   const int rq = 64 * half + 16 * (warp & 3) + (lane >> 2);
   const int cq = 2 * (lane & 3);
   long long c = 0;
@@ -142,6 +145,17 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
     for (int kc = 0; kc < kc_total; ++kc, ++c) {
       const int s = (int)(c % NSTG);
       mbar_wait(bar_full + 8 * s, (uint32_t)((c / NSTG) & 1));
+      {  // round the stage to TF32 in place: this warp group's 64 rows of A, and its half of the W chunk
+        float4* sa = reinterpret_cast<float4*>(smem + s * STG_BYTES + half * (A_BYTES / 2));
+#pragma unroll
+        for (int i = 0; i < (int)(A_BYTES / 2 / 16 / 128); ++i) sa[ct128 + 128 * i] = tf32r4(sa[ct128 + 128 * i]);
+        float4* sw = reinterpret_cast<float4*>(smem + s * STG_BYTES + A_BYTES);
+#pragma unroll
+        for (int i = 0; i < (int)(W_BYTES / 16 / 256); ++i) sw[ct + 256 * i] = tf32r4(sw[ct + 256 * i]);
+        // the rounded values are read by this stage's MMAs (async proxy), and the stage is next overwritten by TMA
+        fence_proxy_async();
+        named_bar_sync(1, 256);  // both consumer warp groups: the whole W chunk is rounded
+      }
       const uint64_t da = gmma_desc(sbase + s * STG_BYTES + half * (A_BYTES / 2));
       const uint64_t db = gmma_desc(sbase + s * STG_BYTES + A_BYTES);
       wgmma_fence(acc, N / 2);

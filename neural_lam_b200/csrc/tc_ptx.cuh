@@ -177,6 +177,16 @@ __device__ __forceinline__ void wgmma_wait0(float* acc, int n) {
   for (int i = 0; i < n; ++i) asm volatile("" : "+f"(acc[i])::"memory");
 }
 
+// wgmma operands are rounded to TF32 (round to nearest, ties away from zero) in shared memory before the MMA reads them;
+// the MMA would otherwise drop the low 13 mantissa bits (truncation: every product biased toward zero, by about 7e-4
+// relative on average)
+__device__ __forceinline__ float tf32r(float x) {
+  uint32_t u;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
+  return __uint_as_float(u);
+}
+__device__ __forceinline__ float4 tf32r4(float4 v) { return make_float4(tf32r(v.x), tf32r(v.y), tf32r(v.z), tf32r(v.w)); }
+
 // byte offset of 16-byte chunk `ch` (0..7) of row `row` inside a 128B-swizzled [128][32 float] block
 __device__ __forceinline__ uint32_t swz(int row, int ch) { return (uint32_t)(row * 128 + ((ch ^ (row & 7)) << 4)); }
 

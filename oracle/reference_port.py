@@ -19,26 +19,40 @@ import torch
 # available (train_model.py:484-488) = TF32 tensor-core matmuls: both operands rounded to TF32 (10
 # explicit mantissa bits), products accumulated in fp32.  ``tf32_matmul()`` makes ``mlp`` emulate that on
 # the CPU, so that "the error of the reference's own GPU configuration" is a number the tests can state
-# without a GPU run of the reference.
+# without a GPU run of the reference.  In fp64 the operands are rounded to TF32 and the products summed in
+# fp64: a reference for kernels whose only intended rounding is that of their TF32 operands.
+# ``mode="rz"`` (truncation toward zero, what a tensor core does with fp32 bits it is handed unrounded) exists
+# so that tests can tell the two rounding modes apart.
 # --------------------------------------------------------------------------------------------------
-_TF32 = False
+_TF32 = None  # None (exact matmuls) or the rounding mode of the operands: "rna" | "rz"
 
 
 @contextlib.contextmanager
-def tf32_matmul(enabled=True):
+def tf32_matmul(enabled=True, mode="rna"):
     global _TF32
-    old, _TF32 = _TF32, bool(enabled)
+    assert mode in ("rna", "rz"), mode
+    old, _TF32 = _TF32, (mode if enabled else None)
     try:
         yield
     finally:
         _TF32 = old
 
 
-def round_tf32(x):
-    """fp32 -> nearest TF32 value (round half away from zero on the 13 dropped mantissa bits), kept in fp32."""
-    assert x.dtype == torch.float32
-    bits = x.contiguous().view(torch.int32)
-    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
+def round_tf32(x, mode="rna"):
+    """-> x rounded to TF32 (10 explicit mantissa bits), same dtype.  ``"rna"``: to nearest, ties away from zero;
+    ``"rz"``: toward zero.  fp32 rounds on the 13 dropped mantissa bits; fp64 rounds its own value (never through
+    fp32 first)."""
+    assert mode in ("rna", "rz"), mode
+    if x.dtype == torch.float32:
+        bits = x.contiguous().view(torch.int32)
+        if mode == "rna":
+            bits = bits + 0x1000
+        return (bits & ~0x1FFF).view(torch.float32)
+    assert x.dtype == torch.float64, x.dtype
+    m, e = torch.frexp(x)                  # x = m * 2^e, 0.5 <= |m| < 1: 11 significant bits = |m| * 2^11 in [1024, 2048)
+    q = m.abs() * 2048.0
+    q = torch.floor(q + 0.5) if mode == "rna" else torch.floor(q)
+    return torch.ldexp(torch.copysign(q, m), (e - 11).to(torch.float64))
 
 
 # ---------------------------------------------------------------------------
@@ -56,8 +70,8 @@ def mlp(x, params, prefix, hidden_layers=1, layer_norm=True, eps=1e-5):
     for k in range(hidden_layers + 1):
         w = params[f"{prefix}.{2 * k}.weight"].to(h.dtype)
         b = params[f"{prefix}.{2 * k}.bias"].to(h.dtype)
-        if _TF32 and h.dtype == torch.float32:
-            h = round_tf32(h) @ round_tf32(w).t() + b
+        if _TF32 is not None and h.dtype in (torch.float32, torch.float64):
+            h = round_tf32(h, _TF32) @ round_tf32(w, _TF32).t() + b
         else:
             h = h @ w.t() + b
         if k != hidden_layers:
