@@ -181,6 +181,22 @@ int nlam_node_update_step_fwd(const NlamMlp* node_mlp, const NlamMlp* out_mlp, c
                               const float* diff_std, const float* diff_mean, float* new_state, int64_t n_rows, int B,
                               int flags, void* stream);
 
+/* The whole mesh->grid decoder of a forecast step (reference gnn_layers.py:110-157 for the m2g InteractionNet, then
+ * graph/base.py:322-342 and forecasters/autoregressive.py:128-131) in two launches (csrc/fused.cu): the edge projections
+ * P_s = send·W1sᵀ (per batch element) and P_e = edge·W1eᵀ + b1 (once), then one kernel for the edge MLP, the per-receiver
+ * aggregation, the node update rec' = rec + node_mlp([rec | aggr]), output_map and the step epilogue of
+ * nlam_rowmlp_step_fwd.  Neither the aggregate nor rec' goes to HBM.  send (B, n_send, 64), rec (B, n_rec, 64) with batch
+ * strides, edge (E, 64) in CSR edge order shared by the batch (edge_bstride 0, or B = 1).  Covered: TF32 math, H = 64,
+ * hidden_layers = 1, edge MLP 192 -> 64 -> 64 with LayerNorm (sum or mean aggregation, no edge update), node MLP
+ * 128 -> 64 -> 64 with LayerNorm, output_map 64 -> 64 -> D (D < 64, no LayerNorm), uniform in-degree d in {1, 2, 4, 8}.
+ * NLAM_E_UNSUPPORTED otherwise (callers then run nlam_inet_fwd with NLAM_EDGE_ONLY + nlam_node_update_step_fwd).
+ * workspace: at least nlam_decode_workspace_bytes(g, B) bytes. */
+size_t nlam_decode_workspace_bytes(const NlamGraph* g, int B);
+int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp,
+                         const float* send, int64_t send_bstride, const float* rec, int64_t rec_bstride, const float* edge,
+                         int64_t edge_bstride, const float* prev, const float* boundary, const float* bmask,
+                         const float* diff_std, const float* diff_mean, float* new_state, int B, int flags, void* workspace,
+                         size_t ws_bytes, void* stream);
 /* out[b,n,:] = scale_n * sum_{k in [ptr[n],ptr[n+1])} x[b, order ? order[k] : k, :]
  * scale_n = 1 (sum) or 1/max(deg,1) (mean).  Deterministic, CSR order. */
 int nlam_segment_sum(const int32_t* ptr, const int32_t* order, int64_t n_seg, const float* x,

@@ -154,6 +154,12 @@ SYMBOLS = {
         ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int,
         ctypes.c_int, ctypes.c_void_p]),
+    "nlam_decode_workspace_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int]),
+    "nlam_decode_step_fwd": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp),
+        ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+        ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "nlam_memcpy3d_async": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
                                             ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int,
                                             ctypes.c_void_p]),

@@ -66,6 +66,30 @@ extern "C" int nlam_node_update_step_fwd(const NlamMlp* node_mlp, const NlamMlp*
 
 static size_t rup256(size_t n) { return (n + 255) / 256 * 256; }
 
+extern "C" size_t nlam_decode_workspace_bytes(const NlamGraph* g, int B) {
+  if (!g || B < 1) return 0;
+  return rup256(tc_decode_workspace_floats(g, B) * sizeof(float));
+}
+
+extern "C" int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp,
+                                    const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge,
+                                    int64_t edge_bs, const float* prev, const float* boundary, const float* bmask,
+                                    const float* diff_std, const float* diff_mean, float* new_state, int B, int flags,
+                                    void* workspace, size_t ws_bytes, void* stream) {
+  NLAM_REQUIRE(g && edge_mlp && node_mlp && out_mlp && send && rec && edge && prev && diff_std && diff_mean && new_state,
+               NLAM_E_INVALID, "nlam_decode_step_fwd: null argument");
+  NLAM_REQUIRE((boundary == nullptr) || bmask, NLAM_E_INVALID, "nlam_decode_step_fwd: boundary without mask");
+  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean};
+  NLAM_REQUIRE(want_tf32(flags) && tc_decode_supported(g, edge_mlp, node_mlp, out_mlp, flags, send, send_bs, rec, rec_bs, edge,
+                                                       edge_bs, B, new_state, &ep),
+               NLAM_E_UNSUPPORTED, "nlam_decode_step_fwd: graph / shape / math mode not covered by the fused decoder");
+  NLAM_REQUIRE(workspace && ws_bytes >= nlam_decode_workspace_bytes(g, B), NLAM_E_WORKSPACE,
+               "nlam_decode_step_fwd: workspace too small (%zu < %zu bytes; see nlam_decode_workspace_bytes)", ws_bytes,
+               nlam_decode_workspace_bytes(g, B));
+  return tc_decode(g, edge_mlp, node_mlp, out_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, new_state, &ep,
+                   (float*)workspace, (cudaStream_t)stream);
+}
+
 // Workspace layout: [aggregate | path-specific scratch].  Sized per path: the fused H = 64 kernels need only the node
 // projections, the generic tensor-core path its projections / hidden activations / messages, the exact fp32 path the
 // message buffer.

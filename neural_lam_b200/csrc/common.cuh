@@ -125,6 +125,15 @@ bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, cons
                            int64_t n_rows, int B, const float* out, const StepEpilogue* ep);
 int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                 int64_t n_rows, int B, float* out, const StepEpilogue* ep, cudaStream_t st);
+// fused.cu: the whole mesh->grid decoder (edge projections + one kernel for edges, aggregation, node update, output_map and
+// step epilogue) on a uniform in-degree graph; ws holds tc_decode_workspace_floats floats
+bool tc_decode_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp, int flags,
+                         const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs,
+                         int B, const float* out, const StepEpilogue* ep);
+size_t tc_decode_workspace_floats(const NlamGraph* g, int B);
+int tc_decode(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp, int flags,
+              const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B,
+              float* out, const StepEpilogue* ep, float* ws, cudaStream_t st);
 // fused.cu: node update + the next layer's node projections in one kernel (stacks of layers over one node set)
 bool tc_node_proj_supported(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs,
                             const float* aggr, int64_t n_rows, const float* out, const float* proj_out);

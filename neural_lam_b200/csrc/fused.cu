@@ -17,7 +17,7 @@
 // edge output), tc_edge_rmw_kernel (split form, edge tensor updated in place or not written), tc_ell_window_kernel
 // (uniform in-degree edge sets), tc_edge_bcast_kernel (batch-broadcast edge features and receivers, split form),
 // tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
-// epilogue).
+// epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).
 #include "tc_ptx.cuh"
 #include "wgmma_tf32.cuh"
 
@@ -233,8 +233,9 @@ __device__ __forceinline__ void fz_add_rows(float (*v)[16], const float* p0, con
   }
 }
 
-// narrow / full-width row store with the optional forecast-step epilogue
-__device__ __forceinline__ void fz_store_rows(const FzParams& p, float* out, int W, long long n_rows, bool step, float (*v)[16],
+// narrow / full-width row store with the optional forecast-step epilogue (P: FzParams or DecParams)
+template <class P>
+__device__ __forceinline__ void fz_store_rows(const P& p, float* out, int W, long long n_rows, bool step, float (*v)[16],
                                               int b, long long r0, bool valid0, bool valid1) {
   const int cq = 2 * (threadIdx.x & 3);
 #pragma unroll
@@ -423,6 +424,213 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
   }
 }
 
+// ------------------------------------------------------------------------------------ mesh -> grid decoder
+// The whole decoder of a forecast step in one kernel, for a uniform in-degree m2g graph (d in {1, 2, 4, 8}, receiver-sorted,
+// edge features shared by the batch).  Per receiver r of batch element b, with P_e = e·W1eᵀ + b1 and P_s = send·W1sᵀ from
+// one tc_rowlinear_kernel launch before it:
+//   P_r   = rec[b, r]·W1rᵀ                                    (fp32, on chip)
+//   m_k   = LN(SiLU(P_e[k] + P_s[b, src[k]] + P_r)·W2ᵀ + b2)  for the d edges k of r
+//   aggr  = sum (or mean) of the m_k                          (warp shuffles, on chip)
+//   grid' = rec + LN(SiLU([rec | aggr]·Wn1ᵀ + bn1)·Wn2ᵀ + bn2)
+//   new   = step epilogue of SiLU(grid'·Wo1ᵀ + bo1)·Wo2ᵀ + bo2
+// A work item is 64 receivers of one batch element and belongs to one warp group; the two warp groups of a CTA share only
+// the weights and synchronise on their own named barriers, so one group's loads overlap the other's MMAs.  Items run
+// batch-fastest: the B items of one receiver block run at about the same time and read its P_e rows from L2.
+namespace dec {
+using fz::CH_A;
+using fz::CH_W;
+constexpr uint32_t W1R = 0, W2E = W1R + 2 * CH_W, WN1 = W2E + 2 * CH_W, WN2 = WN1 + 4 * CH_W, WO1 = WN2 + 2 * CH_W,
+                   WO2 = WO1 + 2 * CH_W;
+constexpr uint32_t NODE = WO2 + 2 * CH_W;  // 128 x 128 operand: [rec | P_r, then aggr]
+constexpr uint32_t EDGE = NODE + 4 * CH_A;  // 128 x 64 operand: hidden edge activations
+constexpr uint32_t PRM = EDGE + 2 * CH_A;   // b2, gamma, beta (edge MLP) | bn1, bn2, gamma, beta (node MLP) | bo1, bo2
+constexpr uint32_t BYTES = PRM + 9 * 64 * 4 + 1024;  // + alignment slack
+static_assert(BYTES <= 227 * 1024, "decoder shared memory exceeds the sm_90 limit");
+}  // namespace dec
+
+struct DecParams {
+  int B, d, mean, D;          // d: uniform in-degree (the kernel's template argument)
+  long long n_rec, n_blocks;  // receivers; 64-receiver blocks
+  const float* rec;           // (B, n_rec, 64), batch stride rec_bs
+  long long rec_bs;
+  const float* ps;            // P_s (B | 1, n_send, 64), batch stride ps_bs
+  long long ps_bs;
+  const float* pe;            // P_e (E, 64), CSR edge order
+  const int32_t* src;         // sender of CSR edge k
+  FzW w1r, w2e, wn1, wn2, wo1, wo2;
+  const float *b2e, *gamma_e, *beta_e, *bn1, *bn2, *gamma_n, *beta_n, *bo1, *bo2;
+  float eps_e, eps_n;
+  float* out;                 // (B, n_rec, D) new state
+  const float *prev, *bnd, *mask, *dstd, *dmean;
+};
+
+template <int DEG>  // uniform in-degree: 1, 2, 4 or 8
+__global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_constant__ DecParams p) {
+  using namespace fz;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const uint32_t sb = smem_u32(s);
+  uint8_t* sN = s + dec::NODE;
+  uint8_t* sE = s + dec::EDGE;
+  float* prm = reinterpret_cast<float*>(s + dec::PRM);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
+  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // operand row of fragment half 0 (half 1: + 8)
+  const int lr = rq - 64 * wg;                              // the same row within the warp group's 64
+  const int cq = 2 * (lane & 3);
+  const uint32_t aN = sb + dec::NODE + wg * (CH_A / 2), aE = sb + dec::EDGE + wg * (CH_A / 2);
+
+  fz_load_w(s + dec::W1R, p.w1r, 2, tid);
+  fz_load_w(s + dec::W2E, p.w2e, 2, tid);
+  fz_load_w(s + dec::WN1, p.wn1, 4, tid);
+  fz_load_w(s + dec::WN2, p.wn2, 2, tid);
+  fz_load_w(s + dec::WO1, p.wo1, 2, tid);
+  fz_load_w(s + dec::WO2, p.wo2, 2, tid);
+  for (int i = tid; i < 64; i += THREADS) {
+    prm[i] = p.b2e[i];
+    prm[64 + i] = p.gamma_e[i];
+    prm[128 + i] = p.beta_e[i];
+    prm[192 + i] = p.bn1[i];
+    prm[256 + i] = p.bn2[i];
+    prm[320 + i] = p.gamma_n[i];
+    prm[384 + i] = p.beta_n[i];
+    prm[448 + i] = p.bo1[i];
+    prm[512 + i] = i < p.D ? p.bo2[i] : 0.f;
+  }
+  fence_proxy_async();
+  __syncthreads();  // the last CTA-wide barrier: from here on each warp group runs on its own
+
+  const float scale = p.mean ? 1.f / (float)DEG : 1.f;
+  const long long n_items = p.n_blocks * p.B;
+  const long long stride = 2LL * gridDim.x;
+  // Loads run one stage ahead of their use: the next item's receiver rows and sender indices are issued before this
+  // item's node / output GEMMs, each sub-tile's P_e / P_s rows before the previous sub-tile's GEMM.
+  float4 x[8];         // receiver rows of the item: 64 rows x 16 float4 over the warp group's 128 threads
+  int sidx[DEG][2];    // sender of each edge row of the thread, per sub-tile
+  float2 pe[2][8], ps[2][8];
+  auto load_item = [&](long long it) {
+    const int bi = (int)(it % p.B);
+    const long long ri = (it / p.B) * 64;
+    const float* rec = p.rec + (long long)bi * p.rec_bs;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const long long r = ri + 8 * q + (gt >> 4);
+      x[q] = r < p.n_rec ? __ldg(reinterpret_cast<const float4*>(rec + r * 64 + (gt & 15) * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int st = 0; st < DEG; ++st)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int e = st * 64 + lr + 8 * i;  // edge within the item; its receiver is e / DEG
+        sidx[st][i] = ri + e / DEG < p.n_rec ? __ldg(p.src + ri * DEG + e) : -1;
+      }
+  };
+  auto gather = [&](int st, int bi, long long ri) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const bool ok = sidx[st][i] >= 0;
+      const float* pk = p.pe + (ri * DEG + st * 64 + lr + 8 * i) * 64;
+      const float* sk = p.ps + (long long)bi * p.ps_bs + (long long)(ok ? sidx[st][i] : 0) * 64;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        pe[i][j] = ok ? __ldg(reinterpret_cast<const float2*>(pk + 8 * j + cq)) : make_float2(0.f, 0.f);
+        ps[i][j] = ok ? __ldg(reinterpret_cast<const float2*>(sk + 8 * j + cq)) : make_float2(0.f, 0.f);
+      }
+    }
+  };
+  float acc[32];
+  float v[2][16];
+  long long item = 2LL * blockIdx.x + wg;
+  if (item < n_items) load_item(item);
+  for (; item < n_items; item += stride) {
+    const int b = (int)(item % p.B);
+    const long long r0 = (item / p.B) * 64;
+    const float* rec = p.rec + (long long)b * p.rec_bs;
+    gather(0, b, r0);
+    // ---- 1. the item's 64 receiver rows -> node operand chunks 0-1 (TF32)
+    named_bar_sync(bar, 128);  // the previous item's MMAs have finished reading the node operand
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      *reinterpret_cast<float4*>(sN + fz_off(CH_A, 64 * wg + 8 * q + (gt >> 4), (gt & 15) * 4)) = tf32r4(x[q]);
+    fence_proxy_async();
+    named_bar_sync(bar, 128);
+    // ---- 2. P_r = rec·W1rᵀ, kept in fp32 in chunks 2-3 (an addend of the edge pre-activation, not an MMA operand)
+    fz_gemm(acc, aN, sb + dec::W1R, 2);
+    fz_unpack(acc, v, nullptr);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<float2*>(sN + fz_off(CH_A, rq + 8 * i, 64 + 8 * j + cq)) = make_float2(v[i][2 * j], v[i][2 * j + 1]);
+    named_bar_sync(bar, 128);  // every P_r row of the item is visible to the whole warp group
+    // ---- 3. edges: DEG sub-tiles of 64 edges = 64 / DEG receivers each
+#pragma unroll
+    for (int st = 0; st < DEG; ++st) {
+      const int rl0 = (st * 64 + lr) / DEG, rl1 = (st * 64 + lr + 8) / DEG;  // receivers of the two fragment rows
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 pr = *reinterpret_cast<const float2*>(sN + fz_off(CH_A, 64 * wg + (i ? rl1 : rl0), 64 + 8 * j + cq));
+          v[i][2 * j] = silu_fast(pe[i][j].x + ps[i][j].x + pr.x);
+          v[i][2 * j + 1] = silu_fast(pe[i][j].y + ps[i][j].y + pr.y);
+        }
+      if (st + 1 < DEG) gather(st + 1, b, r0);
+      fz_store_op(sE, v, rq, wg);  // its barriers also mean every P_r read of this sub-tile is done
+      fz_gemm(acc, aE, sb + dec::W2E, 2);
+      fz_unpack(acc, v, prm);
+      fz_layernorm(v, prm + 64, prm + 128, p.eps_e);
+      // per-receiver sum: the DEG edges of a receiver are consecutive fragment rows, held by lanes 4, 8 and 16 apart
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int t = 0; t < 16; ++t) {
+          float y = v[i][t];
+          if constexpr (DEG >= 2) y += __shfl_xor_sync(0xffffffffu, y, 4);
+          if constexpr (DEG >= 4) y += __shfl_xor_sync(0xffffffffu, y, 8);
+          if constexpr (DEG >= 8) y += __shfl_xor_sync(0xffffffffu, y, 16);
+          v[i][t] = y * scale;
+        }
+      // aggr (TF32, an operand of the node MLP) over the P_r rows of this sub-tile's receivers, which are read only here
+      if (((lane >> 2) & (DEG - 1)) == 0) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float2*>(sN + fz_off(CH_A, 64 * wg + (i ? rl1 : rl0), 64 + 8 * j + cq)) =
+                make_float2(tf32r(v[i][2 * j]), tf32r(v[i][2 * j + 1]));
+      }
+    }
+    if (item + stride < n_items) load_item(item + stride);
+    fence_proxy_async();
+    named_bar_sync(bar, 128);
+    // ---- 4. node MLP on [rec | aggr] + residual, output_map, step epilogue (as the POST_OUTMLP path of fused_mlp_kernel)
+    fz_gemm(acc, aN, sb + dec::WN1, 4);
+    fz_unpack(acc, v, prm + 192);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sN, v, rq, wg);
+    fz_gemm(acc, aN, sb + dec::WN2, 2);
+    fz_unpack(acc, v, prm + 256);
+    fz_layernorm(v, prm + 320, prm + 384, p.eps_n);
+    const long long ra = r0 + lr;
+    const bool valid0 = ra < p.n_rec, valid1 = ra + 8 < p.n_rec;
+    fz_add_rows(v, valid0 ? rec + ra * 64 : nullptr, valid1 ? rec + (ra + 8) * 64 : nullptr);  // L2-hot since step 1
+    fz_store_op(sN, v, rq, wg);
+    fz_gemm(acc, aN, sb + dec::WO1, 2);
+    fz_unpack(acc, v, prm + 448);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sN, v, rq, wg);
+    fz_gemm(acc, aN, sb + dec::WO2, 2);
+    fz_unpack(acc, v, prm + 512);
+    fz_store_rows(p, p.out, p.D, p.n_rec, true, v, b, ra, valid0, valid1);
+  }
+}
+
 // ------------------------------------------------------------------------------------ host
 static FzW wslice(const float* w, int ld, int rows, int cols) { return FzW{w, ld, rows, cols}; }
 
@@ -531,30 +739,37 @@ int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamR
   return fz_launch(p, "tc_rowmlp_kernel", bytes, st);
 }
 
-// ---- node projections of the split first edge Linear: P_s = x_s·W1sᵀ (B_s batches), P_r = x_r·W1rᵀ + b1 (B_r batches)
-static int fz_projections(const NlamGraph* g, const NlamMlp* em, const float* send, int64_t send_bs, const float* rec,
-                          int64_t rec_bs, int B, float* Ps, float* Pr, cudaStream_t st) {
-  const int Bs = (send_bs == 0 || B == 1) ? 1 : B, Br = (rec_bs == 0 || B == 1) ? 1 : B;
+// ---- two 64 -> 64 row Linears in one launch: out0 = x0·W0ᵀ (B0 batches), out1 = x1·W1ᵀ + b1 (B1 batches); W0, W1 are
+// 64-column slices of the first Linear (in_dim 192) of an edge MLP
+static int fz_rowlin2(const float* x0, int64_t x0_bs, int64_t rows0, int B0, const float* w0, float* out0, const float* x1,
+                      int64_t x1_bs, int64_t rows1, int B1, const float* w1, const float* b1, float* out1, cudaStream_t st) {
   FzParams p;
   memset(&p, 0, sizeof(p));
   p.mode = fz::ROWLIN;
   p.n_src = 1;
-  p.src[0] = FzSrc{send, nullptr, Bs > 1 ? send_bs : 0, 64};
-  p.w1 = wslice(em->w[0] + 64, 192, 64, 64);
+  p.src[0] = FzSrc{x0, nullptr, B0 > 1 ? x0_bs : 0, 64};
+  p.w1 = wslice(w0, 192, 64, 64);
   p.kc1 = 2;
-  p.out = Ps;
+  p.out = out0;
   p.out_w = 64;
-  p.n_rows = g->n_send;
-  p.n_tiles = (int)((g->n_send + 127) / 128);
-  p.B = Bs;
-  p.src1 = FzSrc{rec, nullptr, Br > 1 ? rec_bs : 0, 64};
-  p.w3 = wslice(em->w[0] + 128, 192, 64, 64);
-  p.b1_1 = em->b[0];
-  p.out_1 = Pr;
-  p.n_rows1 = g->n_rec;
-  p.n_tiles1 = (int)((g->n_rec + 127) / 128);
-  p.B1 = Br;
-  return fz_launch(p, "tc_rowlinear_kernel", 8.0 * 64 * ((double)g->n_send * Bs + (double)g->n_rec * Br), st);
+  p.n_rows = rows0;
+  p.n_tiles = (int)((rows0 + 127) / 128);
+  p.B = B0;
+  p.src1 = FzSrc{x1, nullptr, B1 > 1 ? x1_bs : 0, 64};
+  p.w3 = wslice(w1, 192, 64, 64);
+  p.b1_1 = b1;
+  p.out_1 = out1;
+  p.n_rows1 = rows1;
+  p.n_tiles1 = (int)((rows1 + 127) / 128);
+  p.B1 = B1;
+  return fz_launch(p, "tc_rowlinear_kernel", 8.0 * 64 * ((double)rows0 * B0 + (double)rows1 * B1), st);
+}
+
+// ---- node projections of the split first edge Linear: P_s = x_s·W1sᵀ (B_s batches), P_r = x_r·W1rᵀ + b1 (B_r batches)
+static int fz_projections(const NlamGraph* g, const NlamMlp* em, const float* send, int64_t send_bs, const float* rec,
+                          int64_t rec_bs, int B, float* Ps, float* Pr, cudaStream_t st) {
+  const int Bs = (send_bs == 0 || B == 1) ? 1 : B, Br = (rec_bs == 0 || B == 1) ? 1 : B;
+  return fz_rowlin2(send, send_bs, g->n_send, Bs, em->w[0] + 64, Ps, rec, rec_bs, g->n_rec, Br, em->w[0] + 128, em->b[0], Pr, st);
 }
 
 // ---- edge stage: messages, optional edge output, per-receiver aggregate
@@ -783,6 +998,107 @@ int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* re
   p.dstd = ep->std;
   p.dmean = ep->mean;
   return fz_launch(p, "tc_node_out_kernel", 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + 3.0 * D * B), st);
+}
+
+// ---- mesh -> grid decoder: edge projections (tc_rowlinear_kernel) + tc_decode_kernel
+bool tc_decode_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp, int flags,
+                         const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs,
+                         int B, const float* out, const StepEpilogue* ep) {
+  int no = 0;
+  if (flags & (NLAM_PROPAGATION | NLAM_MATH_FP32)) return false;
+  if (!g || B < 1 || g->n_rec < 1 || g->n_edges >= (1LL << 31) - 256) return false;
+  const int d = g->uniform_degree;
+  if (d != 1 && d != 2 && d != 4 && d != 8) return false;
+  if (!tc_edge_supported(g, edge_mlp, flags) || !node_mlp_ok(node_mlp)) return false;
+  if (!mlp_shape_ok(out_mlp, &no) || no >= 64 || out_mlp->in_dim != 64 || out_mlp->ln_gamma) return false;
+  // the kernel reads every bias and LayerNorm parameter: a bias-free Linear or an affine-free LayerNorm is not covered
+  for (const NlamMlp* m : {edge_mlp, node_mlp, out_mlp})
+    if (!m->b[0] || !m->b[1]) return false;
+  if (!edge_mlp->ln_beta || !node_mlp->ln_beta) return false;
+  if (!(edge_bs == 0 || B == 1)) return false;  // edge features shared by the batch: P_e is computed once
+  if (!(aligned16(send) && aligned16(rec) && aligned16(edge) && send_bs % 4 == 0 && rec_bs % 4 == 0 && out)) return false;
+  if (B > 1 && send_bs != 0 && send_bs < g->n_send * 64) return false;
+  return ep && ep->prev && ep->std && ep->mean && (!ep->boundary || ep->mask);
+}
+
+size_t tc_decode_workspace_floats(const NlamGraph* g, int B) {
+  return ((size_t)B * g->n_send + (size_t)g->n_edges) * 64;  // P_s (up to B batches) | P_e
+}
+
+int tc_decode(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp, int flags,
+              const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B,
+              float* out, const StepEpilogue* ep, float* ws, cudaStream_t st) {
+  NLAM_REQUIRE(tc_decode_supported(g, edge_mlp, node_mlp, out_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, out, ep),
+               NLAM_E_UNSUPPORTED, "tc_decode: unsupported shapes");
+  const int Bs = (send_bs == 0 || B == 1) ? 1 : B;
+  float* Ps = ws;
+  float* Pe = ws + (size_t)Bs * g->n_send * 64;
+  // P_s = send·W1sᵀ per batch element, P_e = e·W1eᵀ + b1 once for the whole batch
+  int rc = fz_rowlin2(send, send_bs, g->n_send, Bs, edge_mlp->w[0] + 64, Ps, edge, 0, g->n_edges, 1, edge_mlp->w[0],
+                      edge_mlp->b[0], Pe, st);
+  if (rc) return rc;
+  DecParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = B;
+  p.d = g->uniform_degree;
+  p.mean = (flags & NLAM_AGGR_MEAN) ? 1 : 0;
+  p.D = out_mlp->out_dim[1];
+  p.n_rec = g->n_rec;
+  p.n_blocks = (g->n_rec + 63) / 64;
+  p.rec = rec;
+  p.rec_bs = B > 1 ? rec_bs : 0;
+  p.ps = Ps;
+  p.ps_bs = Bs > 1 ? g->n_send * 64 : 0;
+  p.pe = Pe;
+  p.src = g->src;
+  p.w1r = wslice(edge_mlp->w[0] + 128, 192, 64, 64);
+  p.w2e = wslice(edge_mlp->w[1], 64, 64, 64);
+  p.wn1 = wslice(node_mlp->w[0], 128, 64, 128);
+  p.wn2 = wslice(node_mlp->w[1], 64, 64, 64);
+  p.wo1 = wslice(out_mlp->w[0], 64, 64, 64);
+  p.wo2 = wslice(out_mlp->w[1], 64, p.D, 64);
+  p.b2e = edge_mlp->b[1];
+  p.gamma_e = edge_mlp->ln_gamma;
+  p.beta_e = edge_mlp->ln_beta;
+  p.eps_e = edge_mlp->ln_eps;
+  p.bn1 = node_mlp->b[0];
+  p.bn2 = node_mlp->b[1];
+  p.gamma_n = node_mlp->ln_gamma;
+  p.beta_n = node_mlp->ln_beta;
+  p.eps_n = node_mlp->ln_eps;
+  p.bo1 = out_mlp->b[0];
+  p.bo2 = out_mlp->b[1];
+  p.out = out;
+  p.prev = ep->prev;
+  p.bnd = ep->boundary;
+  p.mask = ep->mask;
+  p.dstd = ep->std;
+  p.dmean = ep->mean;
+  const long long n_items = p.n_blocks * B;
+  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_decode: bad work size");
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  void (*kern)(DecParams) = p.d == 1 ? tc_decode_kernel<1> : p.d == 2 ? tc_decode_kernel<2> : p.d == 4 ? tc_decode_kernel<4>
+                                                                                              : tc_decode_kernel<8>;
+  static unsigned mask[4] = {0, 0, 0, 0};
+  const int di = p.d == 1 ? 0 : p.d == 2 ? 1 : p.d == 4 ? 2 : 3;
+  if (!(mask[di] & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec::BYTES));
+    mask[di] |= 1u << (dev & 31);
+  }
+  const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
+  // algorithmic bytes: receivers, P_s, P_e and the sender indices once, previous / new (/ boundary) state, weights
+  const int D = p.D, Br = (rec_bs != 0 && B > 1) ? B : 1;
+  const double bytes = 256.0 * ((double)g->n_rec * Br + (double)g->n_send * Bs + (double)g->n_edges) + 4.0 * g->n_edges +
+                       4.0 * (double)g->n_rec * D * B * (ep->boundary ? 3 : 2) + (ep->boundary ? 4.0 * g->n_rec : 0.0) +
+                       4.0 * (7 * 64 * 64 + 64 * D + 9 * 64);
+  {
+    ProfScope ps("tc_decode_kernel", st, bytes);
+    kern<<<grid, fz::THREADS, dec::BYTES, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
 }
 
 }  // namespace nlam

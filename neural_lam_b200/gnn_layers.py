@@ -370,13 +370,32 @@ class InteractionNet(nn.Module):
                                                       edge_inplace=inplace, proj_in=proj_in, next_edge_seq=nxt)
         return rec_out, edge_out, proj_out
 
+    def _edge_stage_separable(self):
+        """Can the edge stage of this layer run without its node update, so that a later kernel consumes the aggregate
+        (``aggregate_only``, ``decode_step``)?  Needs an InteractionNet without edge update or halo, in CSR edge order,
+        with H = 64 single-block MLPs."""
+        return not (self._halo is not None or self.update_edges or self.propagation or not self._fusable()
+                    or not self._is_sorted or self.edge_mlp[0].in_features != 192)
+
+    @torch.no_grad()
+    def decode_step(self, send_rep, rec_rep, edge_rep, out_seq, prev, boundary, bmask, diff_std, diff_mean, out_flags=0,
+                    out=None):
+        """Inference-only: this layer (the mesh->grid decoder) chained with ``out_seq`` and the forecast-step epilogue in two
+        launches (``ops.decode_step``); neither the aggregate nor the updated receiver rows go to HBM.  Returns the new state,
+        or None when the layer / graph / call shape has no such path (the caller then runs ``aggregate_only``)."""
+        if not self._edge_stage_separable() or (out_flags & _lib.MATH_FP32):
+            return None
+        self._check_inputs(send_rep, rec_rep, edge_rep)
+        _, (s3, r3, e3) = self._batchify(send_rep, rec_rep, edge_rep)
+        return ops.decode_step(self._graph(r3.device), self.edge_mlp, self.aggr_mlp, out_seq, s3, r3, e3, prev, boundary, bmask,
+                               diff_std, diff_mean, flags=self._flags() | out_flags, out=out)
+
     @torch.no_grad()
     def aggregate_only(self, send_rep, rec_rep, edge_rep):
         """Inference-only: the edge stage of the layer (messages + aggregation) WITHOUT the node update; returns the (B, Nr, H)
         aggregate, or None when this layer / call shape has no such kernel path (the caller then runs ``forward``).  Used to
         chain the node update of the mesh->grid layer with the output MLP in one kernel (``ops.node_update_step``)."""
-        if (self._halo is not None or self.update_edges or self.propagation or not self._fusable() or not self._is_sorted
-                or self.edge_mlp[0].in_features != 192):
+        if not self._edge_stage_separable():
             return None
         self._check_inputs(send_rep, rec_rep, edge_rep)
         _, (s3, r3, e3) = self._batchify(send_rep, rec_rep, edge_rep)

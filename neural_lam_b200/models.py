@@ -217,8 +217,16 @@ class BaseGraphModel(StepPredictor):
         mesh_rep = self.g2m_gnn(grid_emb, self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
         grid_rep = self.encoding_grid_mlp.apply_rows([grid_emb], res=grid_emb)  # base.py:308-310
         mesh_rep = self.process_step(mesh_rep, st)
-        grid_rep = self.m2g_gnn(mesh_rep, grid_rep, self.expand_to_batch(st["m2g_emb"], B))
-        if not torch.is_grad_enabled() and not self.output_std and not self.clamps_output:
+        m2g_emb = self.expand_to_batch(st["m2g_emb"], B)
+        inference = not torch.is_grad_enabled() and not self.output_std and not self.clamps_output
+        if inference and hasattr(self.m2g_gnn, "decode_step"):
+            # the fused decoder, as forward_with_boundary runs it: the eager and the captured step compute the same values
+            fused = self.m2g_gnn.decode_step(mesh_rep, grid_rep, m2g_emb, self.output_map, prev_state, None, None, self.diff_std,
+                                             self.diff_mean, out_flags=self.output_map.nlam_flags)
+            if fused is not None:
+                return fused, None
+        grid_rep = self.m2g_gnn(mesh_rep, grid_rep, m2g_emb)
+        if inference:
             # output_map + rescale (base.py:339) + residual (base.py:342) in one launch where the library fuses it
             fused = ops.rowmlp_step(self.output_map, grid_rep, prev_state, None, None, self.diff_std, self.diff_mean,
                                     flags=self.output_map.nlam_flags)
@@ -253,6 +261,13 @@ class BaseGraphModel(StepPredictor):
         clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
         m2g_emb = self.expand_to_batch(st["m2g_emb"], B)
         if clamp is None and hasattr(self.m2g_gnn, "aggregate_only"):
+            # the whole decoder (edge projections, then edges + aggregation + node update + output_map + step epilogue in one
+            # kernel) where the m2g graph has a uniform in-degree the kernel covers
+            fused = self.m2g_gnn.decode_step(mesh_rep, grid_rep, m2g_emb, self.output_map, prev_state, boundary_state,
+                                             boundary_mask, self.diff_std, self.diff_mean,
+                                             out_flags=self.output_map.nlam_flags, out=out)
+            if fused is not None:
+                return fused
             # node update of the mesh->grid layer + output_map + step epilogue in one kernel: the updated grid
             # representation (which nothing else reads) never goes to HBM
             aggr = self.m2g_gnn.aggregate_only(mesh_rep, grid_rep, m2g_emb)

@@ -473,6 +473,51 @@ def node_update_step(node_seq, out_seq, rec, aggr, prev, boundary, bmask, diff_s
     return out
 
 
+def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, boundary, bmask, diff_std, diff_mean, flags=0,
+                out=None):
+    """The whole mesh->grid decoder of a forecast step in two launches (``nlam_decode_step_fwd``): the edge projections,
+    then one kernel for the messages, the per-receiver aggregation, the node update ``rec + node_seq([rec | aggr])``,
+    ``out_seq`` and the forecast-step epilogue ``bmask*boundary + (1-bmask)*(prev + y*diff_std + diff_mean)``.
+    ``edge_csr``: edge features in CSR edge order, shared by the batch.  Returns None when the library does not fuse this
+    graph / shape / math mode (the caller then runs ``inet_fwd(edge_only=True)`` + ``node_update_step``)."""
+    L = _lib.lib()
+    if flags & _lib.MATH_FP32:
+        return None
+    s, Bs, sbs = as_rows(send)
+    r, Br, rbs = as_rows(rec)
+    e, Be, ebs = as_rows(edge_csr)
+    prev = prev.contiguous()
+    _require_cuda(s, r, e, prev, diff_std, diff_mean, boundary, bmask)
+    B = max(Bs, Br, Be)
+    em, nm, om = mlp_struct(edge_seq), mlp_struct(node_seq), mlp_struct(out_seq)
+    D = om.out_dim[om.n_linear - 1]
+    G = r.shape[-2]
+    if (any(b not in (1, B) for b in (Bs, Br, Be)) or (Be > 1 and ebs != 0) or r.shape[-1] != 64 or s.shape[-1] != 64
+            or e.shape[-1] != 64 or G != graph.n_rec or s.shape[-2] < graph.n_send or e.shape[-2] != graph.n_edges
+            or prev.shape != (B, G, D) or r.device != graph.device):
+        return None
+    if boundary is not None:
+        assert bmask is not None, "decode_step: a boundary state needs its mask"
+        boundary, bmask = boundary.contiguous(), bmask.contiguous()
+        assert boundary.shape == prev.shape and bmask.numel() == G
+    if out is None:
+        out = torch.empty_like(prev)
+    assert out.is_contiguous() and out.shape == prev.shape and out.data_ptr() != prev.data_ptr()
+    dev = r.device
+    ws_bytes = L.nlam_decode_workspace_bytes(graph.handle, B)
+    ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+    with torch.cuda.device(dev):
+        rc = L.nlam_decode_step_fwd(graph.handle, ctypes.byref(em), ctypes.byref(nm), ctypes.byref(om),
+                                    s.data_ptr(), sbs if Bs > 1 else 0, r.data_ptr(), rbs if Br > 1 else 0, e.data_ptr(),
+                                    ebs if Be > 1 else 0, prev.data_ptr(), boundary.data_ptr() if boundary is not None else None,
+                                    bmask.data_ptr() if boundary is not None else None, diff_std.data_ptr(),
+                                    diff_mean.data_ptr(), out.data_ptr(), B, flags, ws.data_ptr(), ws_bytes, _stream_ptr(dev))
+    if rc == _lib.E_UNSUPPORTED:
+        return None
+    _lib.check(rc)
+    return out
+
+
 class RecomputeFn(torch.autograd.Function):
     """Forward = hand-written kernels (``kernel_fn``, run without autograd); backward =
     re-evaluate the same math as a differentiable graph (``torch_fn``: custom gather /
