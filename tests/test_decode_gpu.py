@@ -28,12 +28,14 @@ D = 17
 DECODER = ["tc_rowlinear_kernel", "tc_decode_kernel"]
 
 
-def _setup(ei, ns, nr, B, aggr="sum", boundary=True, seed=0, tailed=False):
+def _setup(ei, ns, nr, B, aggr="sum", boundary=True, seed=0, tailed=False, d_out=D, send_rows=None, bcast=()):
+    """``send_rows``: rows of the sender tensor (default ``ns``); ``bcast``: inputs ("send", "rec") given as a stride-0
+    expansion of one batch element"""
     torch.manual_seed(seed)
     net = nlb.InteractionNet(ei, 64, update_edges=False, aggr=aggr, math="tf32")
-    out_map = make_mlp([64, 64, D], layer_norm=False)
+    out_map = make_mlp([64, 64, d_out], layer_norm=False)
     ne = ei.shape[1]
-    shapes = [(B, ns, 64), (B, nr, 64), (1, ne, 64), (B, nr, D), (B, nr, D)]
+    shapes = [(B, send_rows or ns, 64), (B, nr, 64), (1, ne, 64), (B, nr, d_out), (B, nr, d_out)]
     if tailed:
         _tail_params(net, seed + 1)
         _tail_params(out_map, seed + 2)
@@ -44,9 +46,11 @@ def _setup(ei, ns, nr, B, aggr="sum", boundary=True, seed=0, tailed=False):
                 if p.dim() == 1:
                     p.add_(0.1 * torch.randn_like(p))
         send, rec, edge, prev, bnd = (torch.randn(sh) for sh in shapes)
+    send = send[:1].expand(B, -1, -1) if "send" in bcast else send
+    rec = rec[:1].expand(B, -1, -1) if "rec" in bcast else rec
     gen = torch.Generator().manual_seed(seed + 4)
     mask = (torch.rand(nr, generator=gen) < 0.3).float()
-    std, mean = torch.rand(D, generator=gen) + 0.5, torch.randn(D, generator=gen)
+    std, mean = torch.rand(d_out, generator=gen) + 0.5, torch.randn(d_out, generator=gen)
     return dict(ei=ei, B=B, aggr=aggr, net=net, out_map=out_map, send=send, rec=rec, edge=edge, prev=prev,
                 bnd=bnd if boundary else None, mask=mask if boundary else None, std=std, mean=mean)
 
@@ -65,9 +69,15 @@ def _oracle(c, dev, dtype):
     return new
 
 
+def _to_dev(t):
+    if t is not None and t.dim() == 3 and t.shape[0] > 1 and t.stride(0) == 0:  # a batch broadcast stays one on the device
+        return t[:1].to(DEV).expand_as(t)
+    return t.to(DEV) if t is not None else None
+
+
 def _on_gpu(c):
     net, out_map = c["net"].to(DEV), c["out_map"].to(DEV)
-    g = {k: (c[k].to(DEV) if c[k] is not None else None) for k in ("send", "rec", "edge", "prev", "bnd", "mask", "std", "mean")}
+    g = {k: _to_dev(c[k]) for k in ("send", "rec", "edge", "prev", "bnd", "mask", "std", "mean")}
     return net, out_map, g
 
 
@@ -116,10 +126,9 @@ CASES = [
 ]
 
 
-@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_decode_vs_oracle_and_three_launch_path(case):
-    name, ns, nr, d, B, aggr, boundary = case
-    c = _setup(_ell_graph(ns, nr, d, 2), ns, nr, B, aggr=aggr, boundary=boundary)
+def _check_case(name, c):
+    """the fused decoder on the inputs of ``_setup`` against the fp64 oracle and the three-launch path; a rerun is equal
+    bit for bit and boundary rows are copied exactly"""
     with torch.no_grad():
         want = _oracle(c, "cpu", torch.float64)
         old = torch.backends.cuda.matmul.allow_tf32
@@ -141,9 +150,98 @@ def test_decode_vs_oracle_and_three_launch_path(case):
     assert err <= ABS_TOL, err
     assert err <= max(3 * ref_err, 4e-3), (err, ref_err)
     assert vs_old <= VS_OLD_TOL, vs_old
-    if boundary:  # boundary rows are copied exactly
+    if c["bnd"] is not None:  # boundary rows are copied exactly
         sel = c["mask"].bool()
         assert torch.equal(got.cpu()[:, sel], c["bnd"][:, sel])
+
+
+@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
+def test_decode_vs_oracle_and_three_launch_path(case):
+    name, ns, nr, d, B, aggr, boundary = case
+    _check_case(name, _setup(_ell_graph(ns, nr, d, 2), ns, nr, B, aggr=aggr, boundary=boundary))
+
+
+def _multi_item_shape(B):
+    """Receivers for a decoder call at batch B in which every warp group of tc_decode_kernel runs at least 3 items, the last
+    round is partial and the last 64-receiver block is partial.  Returns (n_rec, n_items, warp groups of the launch)."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    n_blocks = -(-6 * sms // B)  # 3 items for each of 2 warp groups on every SM
+    # a partial last round; an odd item count (odd B) also leaves one warp group of a CTA without a last item
+    while (n_blocks * B) % (2 * sms) == 0 or (B % 2 == 1 and n_blocks % 2 == 0):
+        n_blocks += 1
+    n_items = n_blocks * B
+    grid = min((n_items + 1) // 2, sms)  # as tc_decode launches it: CTAs of two warp groups, at most one per SM
+    return 64 * (n_blocks - 1) + 37, n_items, 2 * grid
+
+
+NS_MULTI = 600
+MULTI_ITEM = [
+    # name, in-degree, B, aggregation
+    ("d1_sum_b5", 1, 5, "sum"),
+    ("d1_mean_b32", 1, 32, "mean"),
+    ("d2_mean_b5", 2, 5, "mean"),
+    ("d2_sum_b32", 2, 32, "sum"),
+    ("d4_sum_b5", 4, 5, "sum"),
+    ("d4_mean_b32", 4, 32, "mean"),
+    ("d8_mean_b5", 8, 5, "mean"),
+    ("d8_sum_b32", 8, 32, "sum"),
+]
+
+
+@pytest.mark.parametrize("case", MULTI_ITEM, ids=[c[0] for c in MULTI_ITEM])
+def test_decode_multi_item(case):
+    """Every warp group runs several items: the cross-item prefetch of receiver rows and sender indices, the reuse of the
+    warp group's named barriers and shared operands by later items, and a partial receiver block that is not a warp
+    group's first item.  Items run batch-fastest (item i: block i / B, batch element i % B) on warp group i % groups."""
+    name, d, B, aggr = case
+    nr, n_items, groups = _multi_item_shape(B)
+    assert n_items // groups >= 3, (n_items, groups)  # the fewest items a warp group runs
+    assert n_items % groups != 0 and nr % 64 != 0 and n_items - B >= groups, (nr, n_items, groups)
+    assert B % 2 == 0 or n_items % 2 == 1
+    print(f"\n{name}: {nr} receivers, {n_items} items on {groups} warp groups")
+    _check_case(name, _setup(_ell_graph(NS_MULTI, nr, d, 4), NS_MULTI, nr, B, aggr=aggr))
+
+
+@pytest.mark.parametrize("B", [5, 32])
+def test_decode_multi_item_batch_permutation(B):
+    """Permuting the batch permutes the output bit for bit (the decoder has no reduction across the batch)."""
+    nr, _, _ = _multi_item_shape(B)
+    c = _setup(_ell_graph(NS_MULTI, nr, 4, 5), NS_MULTI, nr, B)
+    perm = torch.arange(B).flip(0).roll(2)
+    assert not torch.equal(perm, torch.arange(B))
+    got, names = _fused(c)
+    assert names == DECODER, names
+    got_p, _ = _fused(dict(c, **{k: c[k][perm] for k in ("send", "rec", "prev", "bnd")}))
+    want = got[perm.to(DEV)]
+    bad = [b for b in range(B) if not torch.equal(got_p[b], want[b])]
+    assert not bad, f"permuted positions {bad} differ (max |diff| {(got_p - want).abs().max().item():.3e})"
+
+
+CALL_SHAPES = [
+    # name, options of _setup
+    ("bcast_send", dict(bcast=("send",))),
+    ("bcast_rec", dict(bcast=("rec",))),
+    ("bcast_send_rec", dict(bcast=("send", "rec"))),
+    ("send_rows_n_send_plus_37", dict(send_rows=300 + 37)),
+    ("d_out_1", dict(d_out=1)),
+    ("d_out_63", dict(d_out=63)),
+]
+
+
+@pytest.mark.parametrize("case", CALL_SHAPES, ids=[c[0] for c in CALL_SHAPES])
+def test_decode_call_shapes(case):
+    """Call shapes tc_decode handles with code of its own: stride-0 senders (one P_s for the batch) and receivers (P_r and
+    the residual from one element), a sender tensor with more rows than the graph's senders, and the narrowest and widest
+    output the kernel accepts (D < 64; columns >= D of the last bias are zero-padded)."""
+    name, kw = case
+    ns, nr, B = 300, 777, 5
+    c = _setup(_ell_graph(ns, nr, 4, 6), ns, nr, B, **kw)
+    _check_case(name, c)
+    _, _, g = _on_gpu(c)
+    for k in kw.get("bcast", ()):
+        assert g[k].stride(0) == 0, k
+    assert c["net"]._graph(g["rec"].device).n_send == ns
+    assert g["send"].shape[1] == kw.get("send_rows", ns) and g["prev"].shape[2] == kw.get("d_out", D)
 
 
 @pytest.mark.parametrize("kind", ["degree3", "non_uniform", "halo"])
