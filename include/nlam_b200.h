@@ -197,6 +197,24 @@ int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
                          int64_t edge_bstride, const float* prev, const float* boundary, const float* bmask,
                          const float* diff_std, const float* diff_mean, float* new_state, int B, int flags, void* workspace,
                          size_t ws_bytes, void* stream);
+/* The grid side of a forecast step's encoder (reference graph/base.py:275-310) in one launch (csrc/fused.cu).  For the
+ * concatenated inputs x = [src_0 | src_1 | ...] (at most 64 columns, dense rows without index) of each grid row:
+ *   grid_emb = embed_mlp(x)                          never leaves the SM
+ *   P_s      = grid_emb·W1sᵀ                         W1s = columns 64..127 of the g2m edge MLP's first Linear
+ *   grid_rep = grid_emb + grid_mlp(grid_emb)
+ * and once for the batch P_r = mesh·W1rᵀ + b1 (W1r = columns 128..191; mesh (g2m receivers, 64) shared by the batch).
+ * grid_rep (B, n_rows, 64) dense; proj = [P_s (B, n_rows, 64) | P_r (n_rec, 64)], 16-byte aligned: the proj_in of the g2m call
+ * nlam_inet_fwd_chain(g2m, ..., send = P_s, rec = mesh, edge = g2m_edge, next_edge_mlp = NULL, proj_in = proj), whose edge
+ * stage then skips its own projection pass.  Covered: TF32 math, H = 64, every MLP in -> 64 -> 64 with biases and an affine
+ * LayerNorm, g2m senders = the n_rows grid rows, and a g2m call that takes the batch-broadcast split edge path (edge features
+ * and mesh rows shared by the batch); nlam_encode_supported says whether a call is.  NLAM_E_UNSUPPORTED otherwise (callers
+ * then run nlam_rowmlp_fwd for the embedder, nlam_inet_fwd for g2m and nlam_rowmlp_fwd for grid_mlp). */
+int nlam_encode_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
+                          const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge,
+                          int64_t edge_bstride, const float* grid_rep, const float* proj, int64_t n_rows, int B, int flags);
+int nlam_encode_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
+                    const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge, int64_t edge_bstride,
+                    float* grid_rep, float* proj, int64_t n_rows, int B, int flags, void* stream);
 /* out[b,n,:] = scale_n * sum_{k in [ptr[n],ptr[n+1])} x[b, order ? order[k] : k, :]
  * scale_n = 1 (sum) or 1/max(deg,1) (mean).  Deterministic, CSR order. */
 int nlam_segment_sum(const int32_t* ptr, const int32_t* order, int64_t n_seg, const float* x,

@@ -160,6 +160,14 @@ SYMBOLS = {
         ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "nlam_encode_supported": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamRowSrc), ctypes.c_int, ctypes.POINTER(NlamMlp),
+        ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
+    "nlam_encode_fwd": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamRowSrc), ctypes.c_int, ctypes.POINTER(NlamMlp),
+        ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "nlam_memcpy3d_async": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
                                             ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int,
                                             ctypes.c_void_p]),

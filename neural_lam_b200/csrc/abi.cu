@@ -144,6 +144,41 @@ static bool chain_path(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMl
   return true;
 }
 
+// grid -> mesh call (batch-broadcast edge features and receivers, no edge update): does nlam_inet_fwd take the split
+// tc_edge_bcast path, which can consume node projections computed by nlam_encode_fwd?
+static bool bcast_path(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
+                       int64_t rec_bs, const float* edge, int64_t edge_bs, int B, int flags) {
+  if (!(want_tf32(flags) && tc_edge_supported(g, edge_mlp, flags))) return false;
+  const int64_t send_rows = (B > 1 && send_bs > 0) ? send_bs / 64 : g->n_send;
+  if (tc_ell_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, false)) return false;
+  if (tc_edge2_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, B, send_rows)) return false;
+  return tc_edge_bcast_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, false);
+}
+
+extern "C" int nlam_encode_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
+                                     const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bs,
+                                     const float* g2m_edge, int64_t edge_bs, const float* grid_rep, const float* proj,
+                                     int64_t n_rows, int B, int flags) {
+  if (!g2m || !embed_mlp || !srcs || !grid_mlp || !g2m_edge_mlp || !mesh || !g2m_edge || !grid_rep || !proj) return 0;
+  if (B < 1 || g2m->n_send != n_rows || (B > 1 && mesh_bs != 0) || (((uintptr_t)grid_rep | (uintptr_t)proj) & 15)) return 0;
+  if (!tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags)) return 0;
+  // the g2m call that consumes the projections: send = P_s, dense (B, n_rows, 64) at the start of proj
+  return bcast_path(g2m, g2m_edge_mlp, proj, B > 1 ? n_rows * 64 : 0, mesh, mesh_bs, g2m_edge, edge_bs, B, flags) ? 1 : 0;
+}
+
+extern "C" int nlam_encode_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
+                               const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bs,
+                               const float* g2m_edge, int64_t edge_bs, float* grid_rep, float* proj, int64_t n_rows, int B,
+                               int flags, void* stream) {
+  NLAM_REQUIRE(g2m && embed_mlp && srcs && grid_mlp && g2m_edge_mlp && mesh && g2m_edge && grid_rep && proj, NLAM_E_INVALID,
+               "nlam_encode_fwd: null argument");
+  NLAM_REQUIRE(nlam_encode_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, mesh_bs, g2m_edge, edge_bs,
+                                     grid_rep, proj, n_rows, B, flags),
+               NLAM_E_UNSUPPORTED, "nlam_encode_fwd: graph / shape / math mode not covered by the fused encoder");
+  return tc_encode(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags, grid_rep, proj,
+                   proj + (size_t)B * n_rows * 64, (cudaStream_t)stream);
+}
+
 extern "C" int nlam_inet_chain_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp,
                                          const NlamMlp* next_edge_mlp, const float* send, int64_t send_bs, const float* rec,
                                          int64_t rec_bs, int B, int flags) {
@@ -190,8 +225,11 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
                    aggr_mlp->out_dim[aggr_mlp->n_linear - 1] == H,
                NLAM_E_INVALID, "nlam_inet_fwd: MLP widths inconsistent with H=%d", H);
   const bool chained = proj_in || next_mlp;
-  NLAM_REQUIRE(!chained || chain_path(g, edge_mlp, aggr_mlp, next_mlp, send, send_bs, rec, rec_bs, B, flags), NLAM_E_UNSUPPORTED,
-               "nlam_inet_fwd_chain: call shape without a chained path (see nlam_inet_chain_supported)");
+  // projections from nlam_encode_fwd: the grid -> mesh call on the tc_edge_bcast path
+  const bool bcast_proj = proj_in && !next_mlp && !edge_out &&
+                          bcast_path(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, B, flags);
+  NLAM_REQUIRE(!chained || bcast_proj || chain_path(g, edge_mlp, aggr_mlp, next_mlp, send, send_bs, rec, rec_bs, B, flags),
+               NLAM_E_UNSUPPORTED, "nlam_inet_fwd_chain: call shape without a chained path (see nlam_inet_chain_supported)");
   NLAM_REQUIRE(!next_mlp || ((((uintptr_t)rec_out | (uintptr_t)proj_out) & 15) == 0), NLAM_E_INVALID,
                "nlam_inet_fwd_chain: unaligned outputs");
   NLAM_REQUIRE(edge_out != edge || inplace_path(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, B, flags),
@@ -239,7 +277,8 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
     } else if (tc_edge_bcast_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, edge_out != nullptr)) {
       // batch-broadcast edge features and receivers, large sender set, no edge update (grid -> mesh): tile-major
       // K = 192 kernel on raw gathered sender rows (fused.cu)
-      rc = tc_edge_bcast(g, edge_mlp, send, send_bs, rec, rec_bs, edge, aggr, B, flags, st, scratch);
+      rc = tc_edge_bcast(g, edge_mlp, send, send_bs, rec, rec_bs, edge, aggr, B, flags, st,
+                         proj_in ? const_cast<float*>(proj_in) : scratch, proj_in != nullptr);
     } else {
       rc = tc_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st, send_rows);
     }

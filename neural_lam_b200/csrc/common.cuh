@@ -109,8 +109,17 @@ int tc_inet_gen(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr
 // fused.cu: batch-broadcast edge features and receivers, no edge update (grid -> mesh)
 bool tc_edge_bcast_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
                              const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B, bool has_edge_out);
+// (ws: [P_s | P_r] of the split form; have_proj: filled by an earlier kernel, tc_encode)
 int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws);
+                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
+                  bool have_proj);
+// fused.cu: the grid side of the encoder in one kernel: grid embedder on the concatenated sources, the g2m edge MLP's node
+// projections P_s (per batch element) and P_r = mesh·W1rᵀ + b1 (once), and grid_rep = grid_emb + grid_mlp(grid_emb)
+bool tc_encode_supported(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
+                         const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags);
+int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp,
+              const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags, float* grid_rep, float* ps, float* pr,
+              cudaStream_t st);
 // fused.cu: split form, out-of-place edge output
 int tc_edge3(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
              int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,

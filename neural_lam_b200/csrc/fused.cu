@@ -233,6 +233,13 @@ __device__ __forceinline__ void fz_add_rows(float (*v)[16], const float* p0, con
   }
 }
 
+// this thread's 16 columns of one fragment row -> a 64-wide output row
+__device__ __forceinline__ void fz_store_row64(float* row, const float* v) {
+  const int cq = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(row + 8 * j + cq) = make_float2(v[2 * j], v[2 * j + 1]);
+}
+
 // narrow / full-width row store with the optional forecast-step epilogue (P: FzParams or DecParams)
 template <class P>
 __device__ __forceinline__ void fz_store_rows(const P& p, float* out, int W, long long n_rows, bool step, float (*v)[16],
@@ -254,8 +261,7 @@ __device__ __forceinline__ void fz_store_rows(const P& p, float* out, int W, lon
         }
       }
     } else if (W == 64) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(out + o + 8 * j + cq) = make_float2(v[i][2 * j], v[i][2 * j + 1]);
+      fz_store_row64(out + o, v[i]);
     } else {
 #pragma unroll
       for (int t = 0; t < 16; ++t) {
@@ -631,6 +637,196 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_
   }
 }
 
+// ------------------------------------------------------------------------------------ grid encoder
+// The grid side of a forecast step's encoder in one kernel.  Per grid row of batch element b, x = [src_0 | src_1 | ...]
+// zero-padded to 64 columns:
+//   grid_emb = LN(SiLU(x·We1ᵀ + be1)·We2ᵀ + be2)               (fp32, on chip)
+//   P_s      = grid_emb·W1sᵀ                                    the g2m edge MLP's sender projection
+//   grid_rep = grid_emb + LN(SiLU(grid_emb·Wa1ᵀ + ba1)·Wa2ᵀ + ba2)
+// and, by extra work items after the grid ones, P_r = mesh·W1rᵀ + b1 once for the batch.  A work item is 64 rows of one
+// batch element and belongs to one warp group, which synchronises on its own named barriers.  The item's input rows are
+// copied with cp.async into a raw fp32 staging buffer while the previous item's GEMMs run; a dense source's rows of one
+// item are one contiguous span, copied in 16-byte pieces where it starts 16-byte aligned and element by element otherwise.
+namespace enc {
+using fz::CH_A;
+using fz::CH_W;
+constexpr uint32_t WE1 = 0, WE2 = WE1 + 2 * CH_W, W1S = WE2 + 2 * CH_W, WA1 = W1S + 2 * CH_W, WA2 = WA1 + 2 * CH_W,
+                   W1R = WA2 + 2 * CH_W;
+constexpr uint32_t A = W1R + 2 * CH_W;    // 128 x 64 operand, 64 rows per warp group
+constexpr uint32_t STG = A + 2 * CH_A;    // per warp group: 64 rows x at most 64 columns of raw inputs, source by source
+constexpr uint32_t COLS = STG + 2 * 64 * 64 * 4;  // operand column c <- staging float cols[c].x + row * cols[c].y (y = 0: zero)
+constexpr uint32_t PRM = COLS + 64 * 8;   // be1, be2, gamma, beta (embedder) | ba1, ba2, gamma, beta (grid MLP) | b1 (g2m)
+constexpr uint32_t BYTES = PRM + 9 * 64 * 4 + 1024;  // + alignment slack
+static_assert(BYTES <= 227 * 1024, "encoder shared memory exceeds the sm_90 limit");
+}  // namespace enc
+
+struct EncParams {
+  int B, n_src;
+  FzSrc src[4];                 // dense rows (idx NULL, row pitch = dim), batch stride bs (0: shared by the batch)
+  long long n_rows, n_tiles;    // grid rows; 64-row tiles per batch element
+  FzW we1, we2, w1s, wa1, wa2, w1r;
+  const float *be1, *be2, *gamma_e, *beta_e, *ba1, *ba2, *gamma_a, *beta_a, *b1;
+  float eps_e, eps_a;
+  float* grid_rep;              // (B, n_rows, 64)
+  float* ps;                    // (B, n_rows, 64)
+  const float* mesh;            // (n_mesh, 64), shared by the batch
+  float* pr;                    // (n_mesh, 64)
+  long long n_mesh, n_mesh_tiles;
+};
+
+__global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_constant__ EncParams p) {
+  using namespace fz;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const uint32_t sb = smem_u32(s);
+  uint8_t* sA = s + enc::A;
+  float* prm = reinterpret_cast<float*>(s + enc::PRM);
+  int2* cols = reinterpret_cast<int2*>(s + enc::COLS);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
+  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // operand row of fragment half 0 (half 1: + 8)
+  const int lr = rq - 64 * wg;                              // the same row within the warp group's 64
+  const uint32_t aA = sb + enc::A + wg * (CH_A / 2);
+  float* stg = reinterpret_cast<float*>(s + enc::STG) + wg * 64 * 64;
+  const uint32_t stg_u = smem_u32(stg);
+
+  fz_load_w(s + enc::WE1, p.we1, 2, tid);
+  fz_load_w(s + enc::WE2, p.we2, 2, tid);
+  fz_load_w(s + enc::W1S, p.w1s, 2, tid);
+  fz_load_w(s + enc::WA1, p.wa1, 2, tid);
+  fz_load_w(s + enc::WA2, p.wa2, 2, tid);
+  fz_load_w(s + enc::W1R, p.w1r, 2, tid);
+  for (int i = tid; i < 64; i += THREADS) {
+    prm[i] = p.be1[i];
+    prm[64 + i] = p.be2[i];
+    prm[128 + i] = p.gamma_e[i];
+    prm[192 + i] = p.beta_e[i];
+    prm[256 + i] = p.ba1[i];
+    prm[320 + i] = p.ba2[i];
+    prm[384 + i] = p.gamma_a[i];
+    prm[448 + i] = p.beta_a[i];
+    prm[512 + i] = p.b1[i];
+    int2 m = make_int2(0, 0);
+    for (int q = 0, off = 0; q < p.n_src; off += p.src[q].dim, ++q)
+      if (i >= off && i < off + p.src[q].dim) m = make_int2(64 * off + i - off, p.src[q].dim);
+    cols[i] = m;
+  }
+  fence_proxy_async();
+  __syncthreads();  // the last CTA-wide barrier: from here on each warp group runs on its own
+
+  const long long n_grid = p.n_tiles * p.B, n_items = n_grid + p.n_mesh_tiles;
+  const long long stride = 2LL * gridDim.x;
+  const uint64_t pol_stream = policy_evict_first(), pol_shared = policy_evict_normal();
+  // the raw input rows of grid item it -> staging (source q at float 64 * (dim_0 + ... + dim_{q-1}), rows dense)
+  auto issue = [&](long long it) {
+    const int bi = (int)(it / p.n_tiles);
+    const long long row0 = (it - (long long)bi * p.n_tiles) * 64;
+    const int n = (int)min(64LL, p.n_rows - row0);
+    int off = 0;
+    for (int q = 0; q < p.n_src; ++q) {
+      const FzSrc& sq = p.src[q];
+      const float* g = sq.ptr + bi * sq.bs + row0 * sq.dim;
+      const uint32_t dst = stg_u + 4u * 64u * (uint32_t)off;
+      const int ne = n * sq.dim, n16 = ((uintptr_t)g & 15) == 0 ? ne >> 2 : 0;
+      const uint64_t pol = sq.bs ? pol_stream : pol_shared;
+      for (int k = gt; k < n16; k += 128) cp_async_16(dst + 16u * k, g + 4 * k, pol);
+      for (int k = 4 * n16 + gt; k < ne; k += 128) cp_async_4(dst + 4u * k, g + k);
+      off += sq.dim;
+    }
+  };
+  float acc[32];
+  float v[2][16], e[2][16];
+  long long item = 2LL * blockIdx.x + wg;
+  if (item < n_grid) issue(item);
+  for (; item < n_items; item += stride) {
+    if (item >= n_grid) {
+      // ---- P_r = mesh·W1rᵀ + b1 for 64 mesh rows (few items: loaded without staging)
+      const long long row0 = (item - n_grid) * 64;
+      float4 x[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const long long r = row0 + 8 * q + (gt >> 4);
+        x[q] = r < p.n_mesh ? __ldg(reinterpret_cast<const float4*>(p.mesh + r * 64 + (gt & 15) * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      named_bar_sync(bar, 128);  // the previous item's MMAs have finished reading the operand
+#pragma unroll
+      for (int q = 0; q < 8; ++q)
+        *reinterpret_cast<float4*>(sA + fz_off(CH_A, 64 * wg + 8 * q + (gt >> 4), (gt & 15) * 4)) = tf32r4(x[q]);
+      fence_proxy_async();
+      named_bar_sync(bar, 128);
+      fz_gemm(acc, aA, sb + enc::W1R, 2);
+      fz_unpack(acc, v, prm + 512);
+      const long long r0 = row0 + lr;
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+        if (r0 + 8 * i < p.n_mesh) fz_store_row64(p.pr + (r0 + 8 * i) * 64, v[i]);
+      continue;
+    }
+    const int b = (int)(item / p.n_tiles);
+    const long long row0 = (item - (long long)b * p.n_tiles) * 64;
+    const int nrows = (int)min(64LL, p.n_rows - row0);
+    // ---- 1. staged inputs -> operand (TF32, zero-padded columns and rows)
+    cp_async_wait_all();
+    named_bar_sync(bar, 128);  // every thread's copies have landed; the previous item's MMAs are done with the operand
+    for (int g = gt; g < 64 * 16; g += 128) {
+      const int i = g >> 4, c = (g & 15) * 4;
+      float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+      float* px = &x.x;
+      if (i < nrows) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int2 m = cols[c + k];
+          if (m.y) px[k] = stg[m.x + i * m.y];
+        }
+      }
+      *reinterpret_cast<float4*>(sA + fz_off(CH_A, 64 * wg + i, c)) = tf32r4(x);
+    }
+    fence_proxy_async();
+    named_bar_sync(bar, 128);  // the operand is complete and the staging buffer free
+    if (item + stride < n_grid) issue(item + stride);
+    // ---- 2. grid embedder
+    fz_gemm(acc, aA, sb + enc::WE1, 2);
+    fz_unpack(acc, v, prm);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, aA, sb + enc::WE2, 2);
+    fz_unpack(acc, v, prm + 64);
+    fz_layernorm(v, prm + 128, prm + 192, p.eps_e);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) e[i][t] = v[i][t];
+    fz_store_op(sA, v, rq, wg);  // grid_emb: the operand of the next three GEMMs
+    const long long r0 = row0 + lr;
+    const bool valid0 = lr < nrows, valid1 = lr + 8 < nrows;
+    const long long o = ((long long)b * p.n_rows + r0) * 64;
+    // ---- 3. P_s = grid_emb·W1sᵀ
+    fz_gemm(acc, aA, sb + enc::W1S, 2);
+    fz_unpack(acc, v, nullptr);
+    if (valid0) fz_store_row64(p.ps + o, v[0]);
+    if (valid1) fz_store_row64(p.ps + o + 8 * 64, v[1]);
+    // ---- 4. grid_rep = grid_emb + encoding grid MLP(grid_emb)
+    fz_gemm(acc, aA, sb + enc::WA1, 2);
+    fz_unpack(acc, v, prm + 256);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, aA, sb + enc::WA2, 2);
+    fz_unpack(acc, v, prm + 320);
+    fz_layernorm(v, prm + 384, prm + 448, p.eps_a);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] += e[i][t];
+    if (valid0) fz_store_row64(p.grid_rep + o, v[0]);
+    if (valid1) fz_store_row64(p.grid_rep + o + 8 * 64, v[1]);
+  }
+}
+
 // ------------------------------------------------------------------------------------ host
 static FzW wslice(const float* w, int ld, int rows, int cols) { return FzW{w, ld, rows, cols}; }
 
@@ -681,7 +877,8 @@ bool tc_rowmlp_supported(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, 
   if (!mlp_shape_ok(mlp, &nout)) return false;
   int k = 0;
   for (int s = 0; s < n_src; ++s) {
-    if (srcs[s].idx || !aligned16(srcs[s].ptr) || srcs[s].bstride % 4 != 0) return false;
+    // (fz_load_a reads with 16-byte loads only from sources whose width is a multiple of 4)
+    if (srcs[s].idx || !aligned16(srcs[s].ptr) || (srcs[s].dim % 4 == 0 && srcs[s].bstride % 4 != 0)) return false;
     k += srcs[s].dim;
   }
   if (k != mlp->in_dim) return false;
@@ -847,8 +1044,9 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
   p.mode = fz::EDGE;
   p.B = B;
   if (split) {
+    // ws = [P_s (Bs batches) | P_r (Br batches)], computed here or (have_proj) by an earlier kernel
     float* Ps = ws;
-    float* Pr = ws + (size_t)(have_proj ? B : Bs) * g->n_send * 64;
+    float* Pr = ws + (size_t)Bs * g->n_send * 64;
     if (!have_proj) {
       int rc = fz_projections(g, em, send, send_bs, rec, rec_bs, B, Ps, Pr, st);
       if (rc) return rc;
@@ -859,10 +1057,10 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
     p.b1 = nullptr;  // carried by P_r
     p.add[0] = Ps;
     p.add_idx[0] = g->src;
-    p.add_bs[0] = (have_proj ? B : Bs) > 1 ? g->n_send * 64 : 0;
+    p.add_bs[0] = Bs > 1 ? g->n_send * 64 : 0;
     p.add[1] = Pr;
     p.add_idx[1] = g->dst;
-    p.add_bs[1] = (have_proj ? B : Br) > 1 ? g->n_rec * 64 : 0;
+    p.add_bs[1] = Br > 1 ? g->n_rec * 64 : 0;
   } else {
     p.n_src = 3;
     p.src[0] = FzSrc{edge, nullptr, eb, 64};
@@ -913,10 +1111,11 @@ int tc_ell_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, 
 }
 
 int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws) {
+                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
+                  bool have_proj) {
   // split form: the batch-shared receiver projection is computed once, the sender projection once per node (both far fewer
   // rows than the batch's edges), and the edge GEMM has K = 64 instead of gathering K = 192 raw rows per edge and batch
-  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, 0, nullptr, aggr_out, B, flags, st, ws, true, false,
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, 0, nullptr, aggr_out, B, flags, st, ws, true, have_proj,
                  "tc_edge_bcast_kernel");
 }
 
@@ -1095,6 +1294,87 @@ int tc_decode(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_m
   {
     ProfScope ps("tc_decode_kernel", st, bytes);
     kern<<<grid, fz::THREADS, dec::BYTES, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
+}
+
+// ---- grid encoder: grid embedder + g2m node projections + encoding grid MLP (tc_encode_kernel)
+static bool enc_mlp_ok(const NlamMlp* m, int in_max) {  // in -> 64 -> 64 with biases and an affine LayerNorm
+  int no = 0;
+  return mlp_shape_ok(m, &no) && no == 64 && m->in_dim <= in_max && m->b[0] && m->b[1] && m->ln_gamma && m->ln_beta;
+}
+
+bool tc_encode_supported(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
+                         const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags) {
+  if (flags & (NLAM_PROPAGATION | NLAM_MATH_FP32)) return false;
+  if (B < 1 || n_rows < 1 || n_rows >= (1LL << 31) - 256 || n_mesh < 1 || n_src < 1 || n_src > 4) return false;
+  if (!enc_mlp_ok(embed_mlp, 64) || !enc_mlp_ok(grid_mlp, 64) || grid_mlp->in_dim != 64) return false;
+  if (!enc_mlp_ok(g2m_edge_mlp, 192) || g2m_edge_mlp->in_dim != 192) return false;
+  int k = 0;
+  for (int s = 0; s < n_src; ++s) {
+    if (srcs[s].idx || srcs[s].dim < 1 || ((uintptr_t)srcs[s].ptr & 3)) return false;
+    k += srcs[s].dim;
+  }
+  return k == embed_mlp->in_dim && aligned16(mesh);
+}
+
+int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp,
+              const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags, float* grid_rep, float* ps, float* pr,
+              cudaStream_t st) {
+  NLAM_REQUIRE(tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, n_mesh, n_rows, B, flags),
+               NLAM_E_UNSUPPORTED, "tc_encode: unsupported shapes");
+  NLAM_REQUIRE(aligned16(grid_rep) && aligned16(ps) && aligned16(pr), NLAM_E_INVALID, "tc_encode: unaligned outputs");
+  EncParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = B;
+  p.n_src = n_src;
+  double bytes = 0;
+  for (int s = 0; s < n_src; ++s) {
+    p.src[s] = FzSrc{srcs[s].ptr, nullptr, B > 1 ? srcs[s].bstride : 0, srcs[s].dim};
+    bytes += 4.0 * n_rows * srcs[s].dim * ((srcs[s].bstride != 0 && B > 1) ? B : 1);
+  }
+  p.n_rows = n_rows;
+  p.n_tiles = (n_rows + 63) / 64;
+  p.we1 = wslice(embed_mlp->w[0], embed_mlp->in_dim, 64, embed_mlp->in_dim);
+  p.we2 = wslice(embed_mlp->w[1], 64, 64, 64);
+  p.w1s = wslice(g2m_edge_mlp->w[0] + 64, 192, 64, 64);
+  p.wa1 = wslice(grid_mlp->w[0], 64, 64, 64);
+  p.wa2 = wslice(grid_mlp->w[1], 64, 64, 64);
+  p.w1r = wslice(g2m_edge_mlp->w[0] + 128, 192, 64, 64);
+  p.be1 = embed_mlp->b[0];
+  p.be2 = embed_mlp->b[1];
+  p.gamma_e = embed_mlp->ln_gamma;
+  p.beta_e = embed_mlp->ln_beta;
+  p.eps_e = embed_mlp->ln_eps;
+  p.ba1 = grid_mlp->b[0];
+  p.ba2 = grid_mlp->b[1];
+  p.gamma_a = grid_mlp->ln_gamma;
+  p.beta_a = grid_mlp->ln_beta;
+  p.eps_a = grid_mlp->ln_eps;
+  p.b1 = g2m_edge_mlp->b[0];
+  p.grid_rep = grid_rep;
+  p.ps = ps;
+  p.mesh = mesh;
+  p.pr = pr;
+  p.n_mesh = n_mesh;
+  p.n_mesh_tiles = (n_mesh + 63) / 64;
+  const long long n_items = p.n_tiles * B + p.n_mesh_tiles;
+  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_encode: bad work size");
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  static unsigned mask = 0;
+  if (!(mask & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc::BYTES));
+    mask |= 1u << (dev & 31);
+  }
+  const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
+  // algorithmic bytes: the inputs once, grid_rep and P_s, the mesh rows and P_r, the weights
+  bytes += 2.0 * 4.0 * 64 * n_rows * B + 2.0 * 4.0 * 64 * n_mesh + 4.0 * (embed_mlp->in_dim * 64 + 5 * 64 * 64 + 9 * 64);
+  {
+    ProfScope ps_("tc_encode_kernel", st, bytes);
+    tc_encode_kernel<<<grid, fz::THREADS, enc::BYTES, st>>>(p);
   }
   count_launch();
   NLAM_CUDA_OK(cudaGetLastError());

@@ -145,6 +145,9 @@ __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* map, int c0, 
 __device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, uint64_t pol) {
   asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol) : "memory");
 }
+__device__ __forceinline__ void cp_async_4(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
 // arrive on an mbarrier once all cp.async of this thread issued so far have landed (the arrival counts against the
 // barrier's expected count)
 __device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {

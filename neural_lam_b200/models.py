@@ -206,16 +206,32 @@ class BaseGraphModel(StepPredictor):
     def process_step(self, mesh_rep, static):
         raise NotImplementedError
 
+    def _encode(self, prev_state, prev_prev_state, forcing):
+        """Grid embedder, grid -> mesh layer and encoding grid MLP (reference graph/base.py:275-310) ->
+        (static embeddings, mesh_rep, grid_rep)."""
+        B = prev_state.shape[0]
+        # grid feature concat (base.py:275-283) is fused into the embedder kernel
+        sources = [prev_state, prev_prev_state, forcing, self.expand_to_batch(self.grid_static_features, B)]
+        if not torch.is_grad_enabled():
+            # one launch for the embedder, the g2m node projections and the encoding grid MLP where the library covers the
+            # shapes; the grid embedding never goes to HBM.  forward_with_boundary and the no-grad forward both take it, so the
+            # eager and the captured step compute the same values
+            st = self.static_embeddings()
+            fused = self.g2m_gnn.encode_step(self.grid_embedder, self.encoding_grid_mlp, sources,
+                                             self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
+            if fused is not None:
+                return st, fused[0], fused[1]
+        grid_emb = self.grid_embedder.apply_rows(sources)
+        st = self.static_embeddings()
+        mesh_rep = self.g2m_gnn(grid_emb, self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
+        grid_rep = self.encoding_grid_mlp.apply_rows([grid_emb], res=grid_emb)  # base.py:308-310
+        return st, mesh_rep, grid_rep
+
     def forward(self, prev_state, prev_prev_state, forcing):
         """``(B,G,d_state), (B,G,d_state), (B,G,d_forcing) -> (new_state, pred_std|None)``
         (reference graph/base.py:228-344)."""
         B = prev_state.shape[0]
-        # grid feature concat (base.py:275-283) is fused into the embedder kernel
-        grid_emb = self.grid_embedder.apply_rows(
-            [prev_state, prev_prev_state, forcing, self.expand_to_batch(self.grid_static_features, B)])
-        st = self.static_embeddings()
-        mesh_rep = self.g2m_gnn(grid_emb, self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
-        grid_rep = self.encoding_grid_mlp.apply_rows([grid_emb], res=grid_emb)  # base.py:308-310
+        st, mesh_rep, grid_rep = self._encode(prev_state, prev_prev_state, forcing)
         mesh_rep = self.process_step(mesh_rep, st)
         m2g_emb = self.expand_to_batch(st["m2g_emb"], B)
         inference = not torch.is_grad_enabled() and not self.output_std and not self.clamps_output
@@ -252,11 +268,7 @@ class BaseGraphModel(StepPredictor):
         into the step epilogue kernel.  ``out``: optional preallocated (B,G,d) tensor for the new state."""
         assert not self.output_std
         B = prev_state.shape[0]
-        grid_emb = self.grid_embedder.apply_rows(
-            [prev_state, prev_prev_state, forcing, self.expand_to_batch(self.grid_static_features, B)])
-        st = self.static_embeddings()
-        mesh_rep = self.g2m_gnn(grid_emb, self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
-        grid_rep = self.encoding_grid_mlp.apply_rows([grid_emb], res=grid_emb)
+        st, mesh_rep, grid_rep = self._encode(prev_state, prev_prev_state, forcing)
         mesh_rep = self.process_step(mesh_rep, st)
         clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
         m2g_emb = self.expand_to_batch(st["m2g_emb"], B)

@@ -518,6 +518,45 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
     return out
 
 
+def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=0):
+    """The grid side of a forecast step's encoder in ONE launch (``nlam_encode_fwd``): ``grid_emb = embed_seq(cat sources)``
+    stays on chip; returns ``(grid_rep, proj)`` with ``grid_rep = grid_emb + grid_seq(grid_emb)`` (B, G, 64) and
+    ``proj = [P_s | P_r]`` flat, ``P_s = grid_emb·W1sᵀ`` (B, G, 64) and ``P_r = mesh·W1rᵀ + b1`` (n_mesh, 64) of the grid -> mesh
+    layer's edge MLP ``edge_seq`` on ``graph`` — the ``proj_in`` of that layer's ``inet_fwd`` with send = P_s.  ``mesh`` and
+    ``edge_csr`` are shared by the batch.  Returns None when the library does not fuse these shapes / this math mode (the
+    caller then runs the embedder, the g2m layer and ``grid_seq`` as three calls)."""
+    L = _lib.lib()
+    if flags & _lib.MATH_FP32:
+        return None
+    prepared = [as_rows(t) for t in sources]
+    m, Bm, mbs = as_rows(mesh)
+    e, Be, ebs = as_rows(edge_csr)
+    _require_cuda(m, e, *[t for t, _, _ in prepared])
+    B = max(b for _, b, _ in prepared)
+    G = prepared[0][0].shape[-2]
+    if (any(b not in (1, B) for _, b, _ in prepared) or any(t.shape[-2] != G for t, _, _ in prepared)
+            or Bm not in (1, B) or Be not in (1, B) or m.shape[-1] != 64 or e.shape[-1] != 64
+            or m.shape[-2] != graph.n_rec or e.shape[-2] != graph.n_edges or m.device != graph.device):
+        return None
+    arr = (NlamRowSrc * len(prepared))()
+    for i, (t, _, bs) in enumerate(prepared):
+        arr[i].ptr = t.data_ptr()
+        arr[i].idx = None
+        arr[i].bstride = bs
+        arr[i].dim = t.shape[-1]
+    em, gm, sm = mlp_struct(embed_seq), mlp_struct(grid_seq), mlp_struct(edge_seq)
+    grid_rep = torch.empty((B, G, 64), device=m.device, dtype=torch.float32)
+    proj = torch.empty((B * G + graph.n_rec) * 64, device=m.device, dtype=torch.float32)
+    with torch.cuda.device(m.device):
+        rc = L.nlam_encode_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
+                               m.data_ptr(), mbs if Bm > 1 else 0, e.data_ptr(), ebs if Be > 1 else 0, grid_rep.data_ptr(),
+                               proj.data_ptr(), G, B, flags, _stream_ptr(m.device))
+    if rc == _lib.E_UNSUPPORTED:
+        return None
+    _lib.check(rc)
+    return grid_rep, proj
+
+
 class RecomputeFn(torch.autograd.Function):
     """Forward = hand-written kernels (``kernel_fn``, run without autograd); backward =
     re-evaluate the same math as a differentiable graph (``torch_fn``: custom gather /
