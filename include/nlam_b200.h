@@ -215,6 +215,27 @@ int nlam_encode_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const 
 int nlam_encode_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
                     const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge, int64_t edge_bstride,
                     float* grid_rep, float* proj, int64_t n_rows, int B, int flags, void* stream);
+/* nlam_encode_fwd that also stores grid_emb (B, n_rows, 64) dense, 16-byte aligned: Graph-EFM's decoder reads it as the
+ * senders of its grid -> mesh layer (reference latent/base_decoder.py:145-155).  Same coverage as nlam_encode_fwd. */
+int nlam_encode_emb_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
+                        const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge,
+                        int64_t edge_bstride, float* grid_rep, float* proj, float* grid_emb, int64_t n_rows, int B, int flags,
+                        void* stream);
+/* The stochastic step of Graph-EFM (reference latent/graph_encoder.py:102-105, base_encoder.py:85-94,
+ * base_decoder.py:145) in one launch (csrc/fused.cu).  Per row r of batch element b, x (B, n_rows, 64) the prior's mesh
+ * representation and eps (B, n_rows, 64) standard normal noise, both with dense rows and batch strides x_bstride /
+ * eps_bstride (floats):
+ *   p          = param_mlp(x)                         latent_param_map: Linear-SiLU-Linear, no LayerNorm, 64 or 128 outputs
+ *   mean, std  = p[:, :64], 1 (64 outputs) or 1e-4 + softplus(p[:, 64:]) (128 outputs)
+ *   z          = mean + eps*std                       torch's rounding: the product, then the sum
+ *   latent_emb = embed_mlp(z)                         latent_embedder: 64 -> 64 -> 64 with LayerNorm
+ * Only latent_emb (B, n_rows, 64) dense is written.  Covered: TF32 math, H = latent_dim = 64, hidden_layers = 1, 16-byte
+ * aligned tensors; nlam_latent_sample_supported says whether a call is.  NLAM_E_UNSUPPORTED otherwise (callers then run
+ * param_mlp, the sample and embed_mlp as separate calls). */
+int nlam_latent_sample_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bstride,
+                                 const float* eps, int64_t eps_bstride, const float* latent_emb, int64_t n_rows, int B, int flags);
+int nlam_latent_sample_fwd(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bstride, const float* eps,
+                           int64_t eps_bstride, float* latent_emb, int64_t n_rows, int B, int flags, void* stream);
 /* out[b,n,:] = scale_n * sum_{k in [ptr[n],ptr[n+1])} x[b, order ? order[k] : k, :]
  * scale_n = 1 (sum) or 1/max(deg,1) (mean).  Deterministic, CSR order. */
 int nlam_segment_sum(const int32_t* ptr, const int32_t* order, int64_t n_seg, const float* x,

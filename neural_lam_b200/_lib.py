@@ -168,6 +168,16 @@ SYMBOLS = {
         ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamRowSrc), ctypes.c_int, ctypes.POINTER(NlamMlp),
         ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
         ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "nlam_encode_emb_fwd": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamRowSrc), ctypes.c_int, ctypes.POINTER(NlamMlp),
+        ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "nlam_latent_sample_supported": (ctypes.c_int, [
+        ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
+        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
+    "nlam_latent_sample_fwd": (ctypes.c_int, [
+        ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
+        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "nlam_memcpy3d_async": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
                                             ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int,
                                             ctypes.c_void_p]),

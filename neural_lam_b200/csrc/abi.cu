@@ -176,7 +176,37 @@ extern "C" int nlam_encode_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, c
                                      grid_rep, proj, n_rows, B, flags),
                NLAM_E_UNSUPPORTED, "nlam_encode_fwd: graph / shape / math mode not covered by the fused encoder");
   return tc_encode(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags, grid_rep, proj,
-                   proj + (size_t)B * n_rows * 64, (cudaStream_t)stream);
+                   proj + (size_t)B * n_rows * 64, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int nlam_encode_emb_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
+                                   const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bs,
+                                   const float* g2m_edge, int64_t edge_bs, float* grid_rep, float* proj, float* grid_emb,
+                                   int64_t n_rows, int B, int flags, void* stream) {
+  NLAM_REQUIRE(g2m && embed_mlp && srcs && grid_mlp && g2m_edge_mlp && mesh && g2m_edge && grid_rep && proj && grid_emb,
+               NLAM_E_INVALID, "nlam_encode_emb_fwd: null argument");
+  NLAM_REQUIRE(((uintptr_t)grid_emb & 15) == 0, NLAM_E_INVALID, "nlam_encode_emb_fwd: unaligned grid_emb");
+  NLAM_REQUIRE(nlam_encode_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, mesh_bs, g2m_edge, edge_bs,
+                                     grid_rep, proj, n_rows, B, flags),
+               NLAM_E_UNSUPPORTED, "nlam_encode_emb_fwd: graph / shape / math mode not covered by the fused encoder");
+  return tc_encode(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags, grid_rep, proj,
+                   proj + (size_t)B * n_rows * 64, grid_emb, (cudaStream_t)stream);
+}
+
+extern "C" int nlam_latent_sample_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs,
+                                            const float* eps, int64_t eps_bs, const float* latent_emb, int64_t n_rows, int B,
+                                            int flags) {
+  if (!param_mlp || !embed_mlp) return 0;
+  return tc_latent_supported(param_mlp, embed_mlp, x, x_bs, eps, eps_bs, latent_emb, n_rows, B, flags) ? 1 : 0;
+}
+
+extern "C" int nlam_latent_sample_fwd(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs,
+                                      const float* eps, int64_t eps_bs, float* latent_emb, int64_t n_rows, int B, int flags,
+                                      void* stream) {
+  NLAM_REQUIRE(param_mlp && embed_mlp && x && eps && latent_emb, NLAM_E_INVALID, "nlam_latent_sample_fwd: null argument");
+  NLAM_REQUIRE(nlam_latent_sample_supported(param_mlp, embed_mlp, x, x_bs, eps, eps_bs, latent_emb, n_rows, B, flags),
+               NLAM_E_UNSUPPORTED, "nlam_latent_sample_fwd: shape / math mode not covered by the fused latent kernel");
+  return tc_latent(param_mlp, embed_mlp, x, x_bs, eps, eps_bs, latent_emb, n_rows, B, flags, (cudaStream_t)stream);
 }
 
 extern "C" int nlam_inet_chain_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp,

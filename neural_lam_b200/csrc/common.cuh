@@ -114,12 +114,18 @@ int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send
                   int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
                   bool have_proj);
 // fused.cu: the grid side of the encoder in one kernel: grid embedder on the concatenated sources, the g2m edge MLP's node
-// projections P_s (per batch element) and P_r = mesh·W1rᵀ + b1 (once), and grid_rep = grid_emb + grid_mlp(grid_emb)
+// projections P_s (per batch element) and P_r = mesh·W1rᵀ + b1 (once), and grid_rep = grid_emb + grid_mlp(grid_emb);
+// grid_emb itself is stored where grid_emb is not NULL
 bool tc_encode_supported(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
                          const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags);
 int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp,
               const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags, float* grid_rep, float* ps, float* pr,
-              cudaStream_t st);
+              float* grid_emb, cudaStream_t st);
+// fused.cu: Graph-EFM's latent step in one kernel: prior latent_param_map, reparameterised sample, decoder latent_embedder
+bool tc_latent_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs, const float* eps,
+                         int64_t eps_bs, const float* out, int64_t n_rows, int B, int flags);
+int tc_latent(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs, const float* eps, int64_t eps_bs,
+              float* out, int64_t n_rows, int B, int flags, cudaStream_t st);
 // fused.cu: split form, out-of-place edge output
 int tc_edge3(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
              int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,

@@ -647,6 +647,7 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_
 // batch element and belongs to one warp group, which synchronises on its own named barriers.  The item's input rows are
 // copied with cp.async into a raw fp32 staging buffer while the previous item's GEMMs run; a dense source's rows of one
 // item are one contiguous span, copied in 16-byte pieces where it starts 16-byte aligned and element by element otherwise.
+// EMIT_EMB: grid_emb is also stored (B, n_rows, 64): Graph-EFM's decoder reads it as the senders of its g2m layer.
 namespace enc {
 using fz::CH_A;
 using fz::CH_W;
@@ -669,11 +670,13 @@ struct EncParams {
   float eps_e, eps_a;
   float* grid_rep;              // (B, n_rows, 64)
   float* ps;                    // (B, n_rows, 64)
+  float* grid_emb;              // (B, n_rows, 64), EMIT_EMB only
   const float* mesh;            // (n_mesh, 64), shared by the batch
   float* pr;                    // (n_mesh, 64)
   long long n_mesh, n_mesh_tiles;
 };
 
+template <bool EMIT_EMB>
 __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_constant__ EncParams p) {
   using namespace fz;
   extern __shared__ uint8_t smem_raw[];
@@ -802,6 +805,10 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
     const long long r0 = row0 + lr;
     const bool valid0 = lr < nrows, valid1 = lr + 8 < nrows;
     const long long o = ((long long)b * p.n_rows + r0) * 64;
+    if (EMIT_EMB) {
+      if (valid0) fz_store_row64(p.grid_emb + o, e[0]);
+      if (valid1) fz_store_row64(p.grid_emb + o + 8 * 64, e[1]);
+    }
     // ---- 3. P_s = grid_emb·W1sᵀ
     fz_gemm(acc, aA, sb + enc::W1S, 2);
     fz_unpack(acc, v, nullptr);
@@ -824,6 +831,163 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
       for (int t = 0; t < 16; ++t) v[i][t] += e[i][t];
     if (valid0) fz_store_row64(p.grid_rep + o, v[0]);
     if (valid1) fz_store_row64(p.grid_rep + o + 8 * 64, v[1]);
+  }
+}
+
+// ------------------------------------------------------------------------------------ Graph-EFM latent sample
+// The stochastic part of a Graph-EFM step in one kernel.  Per mesh row of batch element b, with x the prior's mesh
+// representation and eps standard normal noise:
+//   p          = SiLU(x·W1ᵀ + b1)·W2ᵀ + b2                the prior's latent_param_map (no LayerNorm)
+//   mean, std  = p[:, :64], 1 (isotropic) | 1e-4 + softplus(p[:, 64:]) (diagonal; torch's threshold 20)
+//   z          = mean + eps·std                           rounded as torch's two ops: the product, then the sum
+//   latent_emb = LN(SiLU(z·W3ᵀ + b3)·W4ᵀ + b4)            the decoder's latent_embedder
+// p and z never leave the SM; z is rounded to TF32 (to nearest) as the operand of W3.  Work items, warp-group ownership and
+// the staging of the next item's rows while this item's GEMMs run are those of tc_encode_kernel; x and eps rows are copied
+// in 16-byte pieces into staging rows padded to 68 floats.
+namespace lat {
+using fz::CH_A;
+using fz::CH_W;
+constexpr int PITCH = 68;
+constexpr uint32_t W1 = 0, W2M = W1 + 2 * CH_W, W2S = W2M + 2 * CH_W, W3 = W2S + 2 * CH_W, W4 = W3 + 2 * CH_W;
+constexpr uint32_t A = W4 + 2 * CH_W;     // 128 x 64 operand, 64 rows per warp group
+constexpr uint32_t STG = A + 2 * CH_A;    // per warp group: 64 x rows | 64 eps rows, PITCH floats each
+constexpr uint32_t PRM = STG + 2 * 2 * 64 * PITCH * 4;  // b1 | b2 (mean) | b2 (std) | b3 | b4 | gamma | beta
+constexpr uint32_t BYTES = PRM + 7 * 64 * 4 + 1024;     // + alignment slack
+static_assert(BYTES <= 227 * 1024, "latent kernel shared memory exceeds the sm_90 limit");
+}  // namespace lat
+
+struct LatParams {
+  int B, diag;
+  long long n_rows, n_tiles;   // mesh rows; 64-row tiles per batch element
+  const float* x;              // (B, n_rows, 64), batch stride x_bs
+  const float* eps;            // (B, n_rows, 64), batch stride eps_bs
+  long long x_bs, eps_bs;
+  FzW w1, w2m, w2s, w3, w4;
+  const float *b1, *b2m, *b2s, *b3, *b4, *gamma, *beta;
+  float ln_eps;
+  float* out;                  // (B, n_rows, 64) dense
+};
+
+__global__ void __launch_bounds__(fz::THREADS, 1) tc_latent_kernel(const __grid_constant__ LatParams p) {
+  using namespace fz;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const uint32_t sb = smem_u32(s);
+  uint8_t* sA = s + lat::A;
+  float* prm = reinterpret_cast<float*>(s + lat::PRM);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
+  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // operand row of fragment half 0 (half 1: + 8)
+  const int lr = rq - 64 * wg;                              // the same row within the warp group's 64
+  const int cq = 2 * (lane & 3);
+  const uint32_t aA = sb + lat::A + wg * (CH_A / 2);
+  float* sx = reinterpret_cast<float*>(s + lat::STG) + wg * 2 * 64 * lat::PITCH;
+  float* se = sx + 64 * lat::PITCH;
+  const uint32_t sx_u = smem_u32(sx), se_u = smem_u32(se);
+
+  fz_load_w(s + lat::W1, p.w1, 2, tid);
+  fz_load_w(s + lat::W2M, p.w2m, 2, tid);
+  if (p.diag) fz_load_w(s + lat::W2S, p.w2s, 2, tid);
+  fz_load_w(s + lat::W3, p.w3, 2, tid);
+  fz_load_w(s + lat::W4, p.w4, 2, tid);
+  for (int i = tid; i < 64; i += THREADS) {
+    prm[i] = p.b1[i];
+    prm[64 + i] = p.b2m[i];
+    prm[128 + i] = p.diag ? p.b2s[i] : 0.f;
+    prm[192 + i] = p.b3[i];
+    prm[256 + i] = p.b4[i];
+    prm[320 + i] = p.gamma[i];
+    prm[384 + i] = p.beta[i];
+  }
+  fence_proxy_async();
+  __syncthreads();  // the last CTA-wide barrier: from here on each warp group runs on its own
+
+  const long long n_items = p.n_tiles * p.B, stride = 2LL * gridDim.x;
+  const uint64_t pol = policy_evict_first();
+  // the x and eps rows of item it -> staging (rows of 64 floats, 16-byte aligned: one span per tensor)
+  auto issue = [&](long long it) {
+    const int bi = (int)(it / p.n_tiles);
+    const long long row0 = (it - (long long)bi * p.n_tiles) * 64;
+    const int n = (int)min(64LL, p.n_rows - row0);
+    const float* gx = p.x + bi * p.x_bs + row0 * 64;
+    const float* ge = p.eps + bi * p.eps_bs + row0 * 64;
+    for (int k = gt; k < n * 16; k += 128) {
+      const uint32_t o = 4u * (uint32_t)((k >> 4) * lat::PITCH + (k & 15) * 4);
+      cp_async_16(sx_u + o, gx + 4 * k, pol);
+      cp_async_16(se_u + o, ge + 4 * k, pol);
+    }
+  };
+  float acc[32];
+  float v[2][16], z[2][16];
+  long long item = 2LL * blockIdx.x + wg;
+  if (item < n_items) issue(item);
+  for (; item < n_items; item += stride) {
+    const int b = (int)(item / p.n_tiles);
+    const long long row0 = (item - (long long)b * p.n_tiles) * 64;
+    const int nrows = (int)min(64LL, p.n_rows - row0);
+    const bool valid0 = lr < nrows, valid1 = lr + 8 < nrows;
+    // ---- 1. staged x -> operand (TF32, zero rows past the end); this thread's eps in the accumulator fragment layout
+    cp_async_wait_all();
+    named_bar_sync(bar, 128);  // every thread's copies have landed; the previous item's MMAs are done with the operand
+    for (int g = gt; g < 64 * 16; g += 128) {
+      const int i = g >> 4, c = (g & 15) * 4;
+      const float4 x = i < nrows ? *reinterpret_cast<const float4*>(sx + i * lat::PITCH + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+      *reinterpret_cast<float4*>(sA + fz_off(CH_A, 64 * wg + i, c)) = tf32r4(x);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 e = (i ? valid1 : valid0) ? *reinterpret_cast<const float2*>(se + (lr + 8 * i) * lat::PITCH + 8 * j + cq)
+                                               : make_float2(0.f, 0.f);
+        z[i][2 * j] = e.x;
+        z[i][2 * j + 1] = e.y;
+      }
+    fence_proxy_async();
+    named_bar_sync(bar, 128);  // the operand is complete and the staging buffers free
+    if (item + stride < n_items) issue(item + stride);
+    // ---- 2. prior latent_param_map: hidden layer
+    fz_gemm(acc, aA, sb + lat::W1, 2);
+    fz_unpack(acc, v, prm);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sA, v, rq, wg);
+    // ---- 3. eps·std (diagonal: std = 1e-4 + softplus(raw); isotropic: std = 1, eps·1 = eps)
+    if (p.diag) {
+      fz_gemm(acc, aA, sb + lat::W2S, 2);
+      fz_unpack(acc, v, prm + 128);
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int t = 0; t < 16; ++t) {
+          const float r = v[i][t];
+          const float sp = r > 20.f ? r : log1pf(expf(r));
+          z[i][t] = __fmul_rn(z[i][t], __fadd_rn(1e-4f, sp));
+        }
+    }
+    // ---- 4. z = mean + eps·std
+    fz_gemm(acc, aA, sb + lat::W2M, 2);
+    fz_unpack(acc, v, prm + 64);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = __fadd_rn(v[i][t], z[i][t]);
+    fz_store_op(sA, v, rq, wg);
+    // ---- 5. decoder latent_embedder
+    fz_gemm(acc, aA, sb + lat::W3, 2);
+    fz_unpack(acc, v, prm + 192);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, aA, sb + lat::W4, 2);
+    fz_unpack(acc, v, prm + 256);
+    fz_layernorm(v, prm + 320, prm + 384, p.ln_eps);
+    const long long o = ((long long)b * p.n_rows + row0 + lr) * 64;
+    if (valid0) fz_store_row64(p.out + o, v[0]);
+    if (valid1) fz_store_row64(p.out + o + 8 * 64, v[1]);
   }
 }
 
@@ -1322,10 +1486,11 @@ bool tc_encode_supported(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n
 
 int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp,
               const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags, float* grid_rep, float* ps, float* pr,
-              cudaStream_t st) {
+              float* grid_emb, cudaStream_t st) {
   NLAM_REQUIRE(tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, n_mesh, n_rows, B, flags),
                NLAM_E_UNSUPPORTED, "tc_encode: unsupported shapes");
-  NLAM_REQUIRE(aligned16(grid_rep) && aligned16(ps) && aligned16(pr), NLAM_E_INVALID, "tc_encode: unaligned outputs");
+  NLAM_REQUIRE(aligned16(grid_rep) && aligned16(ps) && aligned16(pr) && aligned16(grid_emb), NLAM_E_INVALID,
+               "tc_encode: unaligned outputs");
   EncParams p;
   memset(&p, 0, sizeof(p));
   p.B = B;
@@ -1356,6 +1521,7 @@ int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const
   p.b1 = g2m_edge_mlp->b[0];
   p.grid_rep = grid_rep;
   p.ps = ps;
+  p.grid_emb = grid_emb;
   p.mesh = mesh;
   p.pr = pr;
   p.n_mesh = n_mesh;
@@ -1366,15 +1532,84 @@ int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const
   NLAM_CUDA_OK(cudaGetDevice(&dev));
   static unsigned mask = 0;
   if (!(mask & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc::BYTES));
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc::BYTES));
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc::BYTES));
     mask |= 1u << (dev & 31);
   }
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
-  // algorithmic bytes: the inputs once, grid_rep and P_s, the mesh rows and P_r, the weights
-  bytes += 2.0 * 4.0 * 64 * n_rows * B + 2.0 * 4.0 * 64 * n_mesh + 4.0 * (embed_mlp->in_dim * 64 + 5 * 64 * 64 + 9 * 64);
+  // algorithmic bytes: the inputs once, grid_rep and P_s (and grid_emb), the mesh rows and P_r, the weights
+  bytes += (grid_emb ? 3.0 : 2.0) * 4.0 * 64 * n_rows * B + 2.0 * 4.0 * 64 * n_mesh +
+           4.0 * (embed_mlp->in_dim * 64 + 5 * 64 * 64 + 9 * 64);
   {
     ProfScope ps_("tc_encode_kernel", st, bytes);
-    tc_encode_kernel<<<grid, fz::THREADS, enc::BYTES, st>>>(p);
+    if (grid_emb)
+      tc_encode_kernel<true><<<grid, fz::THREADS, enc::BYTES, st>>>(p);
+    else
+      tc_encode_kernel<false><<<grid, fz::THREADS, enc::BYTES, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
+}
+
+// ---- Graph-EFM latent step: latent_param_map + sample + latent_embedder (tc_latent_kernel)
+bool tc_latent_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs, const float* eps,
+                         int64_t eps_bs, const float* out, int64_t n_rows, int B, int flags) {
+  if (flags & (NLAM_PROPAGATION | NLAM_MATH_FP32)) return false;
+  if (B < 1 || n_rows < 1 || n_rows >= (1LL << 31) - 256) return false;
+  // latent_param_map: 64 -> 64 -> 64 (isotropic) or 128 (diagonal), biases, no LayerNorm
+  const NlamMlp* m = param_mlp;
+  if (m->n_linear != 2 || m->in_dim != 64 || m->out_dim[0] != 64 || (m->out_dim[1] != 64 && m->out_dim[1] != 128)) return false;
+  if (m->ln_gamma || !m->b[0] || !m->b[1]) return false;
+  if (!aligned16(m->w[0]) || !aligned16(m->w[1]) || !aligned16(m->b[0]) || !aligned16(m->b[1])) return false;
+  if (!enc_mlp_ok(embed_mlp, 64) || embed_mlp->in_dim != 64) return false;
+  if (!x || !eps || !out || !aligned16(x) || !aligned16(eps) || !aligned16(out)) return false;
+  return x_bs >= 0 && eps_bs >= 0 && x_bs % 4 == 0 && eps_bs % 4 == 0;
+}
+
+int tc_latent(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs, const float* eps, int64_t eps_bs,
+              float* out, int64_t n_rows, int B, int flags, cudaStream_t st) {
+  NLAM_REQUIRE(tc_latent_supported(param_mlp, embed_mlp, x, x_bs, eps, eps_bs, out, n_rows, B, flags), NLAM_E_UNSUPPORTED,
+               "tc_latent: unsupported shapes");
+  LatParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = B;
+  p.diag = param_mlp->out_dim[1] == 128;
+  p.n_rows = n_rows;
+  p.n_tiles = (n_rows + 63) / 64;
+  p.x = x;
+  p.x_bs = B > 1 ? x_bs : 0;
+  p.eps = eps;
+  p.eps_bs = B > 1 ? eps_bs : 0;
+  p.w1 = wslice(param_mlp->w[0], 64, 64, 64);
+  p.w2m = wslice(param_mlp->w[1], 64, 64, 64);
+  p.w2s = wslice(param_mlp->w[1] + 64 * 64, 64, 64, 64);
+  p.w3 = wslice(embed_mlp->w[0], 64, 64, 64);
+  p.w4 = wslice(embed_mlp->w[1], 64, 64, 64);
+  p.b1 = param_mlp->b[0];
+  p.b2m = param_mlp->b[1];
+  p.b2s = param_mlp->b[1] + 64;
+  p.b3 = embed_mlp->b[0];
+  p.b4 = embed_mlp->b[1];
+  p.gamma = embed_mlp->ln_gamma;
+  p.beta = embed_mlp->ln_beta;
+  p.ln_eps = embed_mlp->ln_eps;
+  p.out = out;
+  const long long n_items = p.n_tiles * B;
+  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_latent: bad work size");
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  static unsigned mask = 0;
+  if (!(mask & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_latent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lat::BYTES));
+    mask |= 1u << (dev & 31);
+  }
+  const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
+  // algorithmic bytes: x, eps and latent_emb once, the weights
+  const double bytes = 3.0 * 4.0 * 64 * n_rows * B + 4.0 * ((p.diag ? 5 : 4) * 64 * 64 + (p.diag ? 8 : 7) * 64);
+  {
+    ProfScope ps_("tc_latent_kernel", st, bytes);
+    tc_latent_kernel<<<grid, fz::THREADS, lat::BYTES, st>>>(p);
   }
   count_launch();
   NLAM_CUDA_OK(cudaGetLastError());

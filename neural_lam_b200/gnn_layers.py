@@ -391,11 +391,12 @@ class InteractionNet(nn.Module):
                                diff_std, diff_mean, flags=self._flags() | out_flags, out=out)
 
     @torch.no_grad()
-    def encode_step(self, embedder, grid_mlp, grid_inputs, rec_rep, edge_rep):
+    def encode_step(self, embedder, grid_mlp, grid_inputs, rec_rep, edge_rep, want_grid_emb=False):
         """Inference-only, for the grid -> mesh layer of a forecast step: ``grid_emb = embedder(cat grid_inputs)``, this layer's
         node projections and ``grid_rep = grid_emb + grid_mlp(grid_emb)`` in one launch (``ops.encode``; grid_emb never goes
         to HBM), then this layer's edge stage on those projections and its node update.  Returns ``(rec_rep', grid_rep)``, or
-        None when the layer / graph / call shape has no such path (the caller then runs the three calls)."""
+        None when the layer / graph / call shape has no such path (the caller then runs the three calls).
+        ``want_grid_emb``: the launch also stores grid_emb, returned third (Graph-EFM's decoder reads it)."""
         if not self._edge_stage_separable():
             return None
         _, (r3, e3) = self._batchify(rec_rep, edge_rep)
@@ -403,15 +404,15 @@ class InteractionNet(nn.Module):
             return None
         g = self._graph(r3.device)
         fl = self._flags() | embedder.nlam_flags | grid_mlp.nlam_flags
-        enc = ops.encode(g, embedder, grid_inputs, grid_mlp, self.edge_mlp, r3, e3, flags=fl)
+        enc = ops.encode(g, embedder, grid_inputs, grid_mlp, self.edge_mlp, r3, e3, flags=fl, want_emb=want_grid_emb)
         if enc is None:
             return None
-        grid_rep, proj = enc
+        grid_rep, proj = enc[:2]
         B, G = grid_rep.shape[0], grid_rep.shape[1]
         ps = proj[: B * G * 64].view(B, G, 64)
         rec_out, _, _, _ = ops.inet_fwd(g, self.edge_mlp, self.aggr_mlp, ps, r3.expand(B, -1, -1), e3.expand(B, -1, -1), False,
                                         self._flags(), proj_in=proj)
-        return rec_out, grid_rep
+        return (rec_out, grid_rep, enc[2]) if want_grid_emb else (rec_out, grid_rep)
 
     @torch.no_grad()
     def aggregate_only(self, send_rep, rec_rep, edge_rep):

@@ -25,6 +25,7 @@ from torch import nn
 from . import _lib, ops
 from .gnn_layers import InteractionNet, get_gnn_class
 from . import clamping
+from .latent import ConstantLatentEncoder, GraphLatentDecoder, GraphLatentEncoder
 from .clamping import OutputClamp
 from .networks import GNNSequential, make_mlp
 from .synthetic import normalize_graph
@@ -509,6 +510,204 @@ class HiLAMParallel(BaseHiGraphModel):
         return levels, list(sections[:L]), list(sections[L:2 * L - 1]), list(sections[2 * L - 1:])
 
 
+class GraphEFMMultiScale(BaseGraphModel):
+    """Graph-EFM, the latent-variable ensemble forecaster, on a flat (multiscale) mesh (reference
+    step_predictors/graph/graph_efm.py: BaseGraphEFM :25-471, GraphEFMMultiScale :796-1037).  ``forward`` samples one step
+    from the prior: grid embedding, prior over a latent on the mesh nodes, reparameterised sample, decoder.  The
+    variational posterior is ``self.encoder`` (conditioned on the target through ``embedd_grid_with_target``); the
+    predictor computes no loss.
+
+    Submodule names and persistent buffers are the reference's, so its state_dicts load strictly.  The graph registration
+    and the cache of the weight-only embeddings are ``BaseGraphModel``'s; the encode-process-decode modules of
+    ``BaseGraphModel.__init__`` are not built (``StepPredictor.__init__`` runs instead).
+
+    Noise: ``latent_noise`` (B, N_mesh, latent_dim) is the standard normal ε of ``z = mean + ε * std``; without it ε is
+    drawn with ``torch.randn`` on the default generator of the current device.  Under autograd the sample is composed from
+    the module outputs in that order; the no-grad step runs the fused kernels where they cover the shapes."""
+
+    samples_latent = True
+
+    def __init__(self, datastore, graph, hidden_dim=64, hidden_layers=1, latent_dim=None, prior_m2m_layers=2,
+                 encoder_m2m_layers=2, decoder_m2m_layers=4, learn_prior=True, prior_dist="isotropic",
+                 g2m_gnn_type="InteractionNet", m2g_gnn_type="InteractionNet", output_std=False,
+                 output_clamping_lower=None, output_clamping_upper=None, math=None):
+        StepPredictor.__init__(self, datastore, output_std=output_std, output_clamping_lower=output_clamping_lower,
+                               output_clamping_upper=output_clamping_upper)
+        self.g2m_gnn_type, self.m2g_gnn_type = g2m_gnn_type, m2g_gnn_type
+        self.register_buffer("diff_mean", datastore.state_diff_mean.float(), persistent=False)
+        self.register_buffer("diff_std", datastore.state_diff_std.float(), persistent=False)
+        self.hidden_dim, self.hidden_layers, self.math = hidden_dim, hidden_layers, math
+        g = graph if graph.get("normalized") else normalize_graph(graph)
+        self.hierarchical = bool(g["hierarchical"])
+        if self.hierarchical:
+            raise ValueError(f"{type(self).__name__} requires a flat mesh graph, but the graph is hierarchical")
+        self._register_graph(g)
+        self.num_mesh_nodes, _ = self.get_num_mesh()
+        self.grid_input_dim = self.grid_dim = datastore.grid_input_dim
+        g2m_dim, m2g_dim = self.g2m_features.shape[1], self.m2g_features.shape[1]
+
+        self.mlp_blueprint_end = [hidden_dim] * (hidden_layers + 1)
+        self.grid_prev_embedder = make_mlp([self.grid_dim] + self.mlp_blueprint_end)
+        self.grid_current_embedder = make_mlp([self.grid_dim + self.num_state_vars] + self.mlp_blueprint_end)
+        self.g2m_embedder = make_mlp([g2m_dim] + self.mlp_blueprint_end)
+        self.m2g_embedder = make_mlp([m2g_dim] + self.mlp_blueprint_end)
+        self.latent_dim = latent_dim if latent_dim is not None else hidden_dim
+        if learn_prior:
+            self.prior_model = GraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, hidden_dim,
+                                                  prior_m2m_layers, hidden_layers=hidden_layers, g2m_gnn_type=g2m_gnn_type,
+                                                  output_dist=prior_dist, math=math)
+        else:
+            self.prior_model = ConstantLatentEncoder(self.latent_dim, self.num_mesh_nodes, output_dist=prior_dist)
+        self.mesh_embedder = make_mlp([self.mesh_static_features.shape[1]] + self.mlp_blueprint_end)
+        self.m2m_embedder = make_mlp([self.m2m_features.shape[1]] + self.mlp_blueprint_end)
+        self.encoder = GraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, hidden_dim,
+                                          encoder_m2m_layers, hidden_layers=hidden_layers, g2m_gnn_type=g2m_gnn_type,
+                                          output_dist="diagonal", math=math)
+        self.decoder = GraphLatentDecoder(self.g2m_edge_index, self.m2m_edge_index, self.m2g_edge_index, hidden_dim,
+                                          self.latent_dim, self.num_state_vars, decoder_m2m_layers, hidden_layers=hidden_layers,
+                                          g2m_gnn_type=g2m_gnn_type, m2g_gnn_type=m2g_gnn_type, output_std=bool(output_std),
+                                          math=math)
+        self._static_cache = None
+        self._set_mlp_flags()
+
+    def get_num_mesh(self):
+        return self.mesh_static_features.shape[0], 0
+
+    @property
+    def latent_spatial_dim(self):
+        return self.num_mesh_nodes
+
+    def _static_params(self):
+        return [p for m in (self.g2m_embedder, self.m2g_embedder, self.mesh_embedder, self.m2m_embedder)
+                for p in m.parameters()]
+
+    def _compute_static(self):
+        return {"g2m_emb": self.g2m_embedder(self.g2m_features), "m2g_emb": self.m2g_embedder(self.m2g_features),
+                "mesh_emb": self.mesh_embedder(self.mesh_static_features),
+                "m2m_emb": self.m2m_embedder(self.m2m_features)}
+
+    def _graph_emb(self, batch_size):
+        st = self.static_embeddings()
+        return {k: self.expand_to_batch(st[f"{k}_emb"], batch_size) for k in ("g2m", "m2g", "mesh", "m2m")}
+
+    def _grid_sources(self, prev_state, prev_prev_state, forcing):
+        # Graph-EFM's order puts X_{t-1} first (graph_efm.py:386-394; GraphLAM puts X_t first)
+        return [prev_prev_state, prev_state, forcing, self.expand_to_batch(self.grid_static_features, prev_state.shape[0])]
+
+    def embedd_mesh(self, batch_size):
+        """``mesh`` and ``m2m`` embeddings expanded to the batch (graph_efm.py:1015-1037)."""
+        ge = self._graph_emb(batch_size)
+        return {"mesh": ge["mesh"], "m2m": ge["m2m"]}
+
+    def embedd_grid_and_graph(self, prev_state, prev_prev_state, forcing):
+        """-> (grid_emb (B, G, H), graph_emb {g2m, m2g, mesh, m2m}) (graph_efm.py:364-413)"""
+        grid_emb = self.grid_prev_embedder.apply_rows(self._grid_sources(prev_state, prev_prev_state, forcing))
+        return grid_emb, self._graph_emb(prev_state.shape[0])
+
+    def embedd_grid_with_target(self, prev_state, prev_prev_state, forcing, current_state):
+        """Grid embedding including the target X_{t+1}, the input of the variational encoder (graph_efm.py:301-343)."""
+        prev_prev, prev, forc, static = self._grid_sources(prev_state, prev_prev_state, forcing)
+        # the row kernels take at most four sources: the last two columns blocks go in as one
+        return self.grid_current_embedder.apply_rows([prev_prev, prev, forc, torch.cat((static, current_state), dim=-1)])
+
+    def _noise(self, latent_noise, batch_size, device):
+        shape = (batch_size, self.num_mesh_nodes, self.latent_dim)
+        if latent_noise is None:
+            return torch.randn(shape, device=device)
+        if tuple(latent_noise.shape) != shape:
+            raise ValueError(f"latent_noise: expected shape {shape}, got {tuple(latent_noise.shape)}")
+        return latent_noise
+
+    def forward(self, prev_state, prev_prev_state, forcing, latent_noise=None):
+        """``(B,G,d_state) x 2, (B,G,d_forcing) -> (new_state, pred_std|None)``: one step sampled from the prior
+        (graph_efm.py:415-471)."""
+        if not torch.is_grad_enabled():
+            return self._step(prev_state, prev_prev_state, forcing, latent_noise, None, None, None)
+        grid_emb, graph_emb = self.embedd_grid_and_graph(prev_state, prev_prev_state, forcing)
+        prior = self.prior_model(grid_emb, graph_emb=graph_emb)
+        eps = self._noise(latent_noise, prev_state.shape[0], prev_state.device)
+        latent_samples = prior.mean + eps * prior.stddev
+        mean_delta, pred_std = self.decoder(grid_emb, latent_samples, graph_emb)
+        rescaled = mean_delta * self.diff_std + self.diff_mean
+        return self.get_clamped_new_state(rescaled, prev_state), pred_std
+
+    @torch.no_grad()
+    def forward_with_boundary(self, prev_state, prev_prev_state, forcing, boundary_state, boundary_mask, latent_noise=None,
+                              out=None):
+        """Inference step with the ARForecaster boundary mix fused into the step epilogue.  ``out``: optional preallocated
+        (B,G,d) tensor for the new state."""
+        assert not self.output_std
+        return self._step(prev_state, prev_prev_state, forcing, latent_noise, boundary_state, boundary_mask, out)[0]
+
+    @torch.no_grad()
+    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
+        """The no-grad step: (1) grid embedder, decoder grid MLP and the prior g2m's projections in one launch, (2) prior g2m,
+        (3) prior m2m stack, (4) prior parameters + sample + latent embedding in one launch, (5) decoder g2m, (6) decoder
+        m2m stack, (7) m2g + param_map + step epilogue.  Each fused launch falls back to its composition where the library
+        does not cover the shapes."""
+        B = prev_state.shape[0]
+        ge = self._graph_emb(B)
+        prior, dec = self.prior_model, self.decoder
+        learned = isinstance(prior, GraphLatentEncoder)
+        sources = self._grid_sources(prev_state, prev_prev_state, forcing)
+        enc = None
+        if learned:
+            enc = prior.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, ge["mesh"], ge["g2m"],
+                                            want_grid_emb=True)
+        if enc is not None:
+            mesh_rep, res_grid, grid_emb = enc
+        else:
+            grid_emb = self.grid_prev_embedder.apply_rows(sources)
+            res_grid = dec.grid_update_mlp.apply_rows([grid_emb], res=grid_emb)
+            mesh_rep = prior.g2m_gnn(grid_emb, ge["mesh"], ge["g2m"]) if learned else None
+        eps = self._noise(latent_noise, B, prev_state.device)
+        latent_emb = None
+        if learned:
+            mesh_rep = prior.process_mesh(mesh_rep, ge["m2m"])
+            latent_emb = ops.latent_sample(prior.latent_param_map, dec.latent_embedder, mesh_rep, eps,
+                                           flags=prior.latent_param_map.nlam_flags | dec.latent_embedder.nlam_flags)
+        if latent_emb is None:
+            dist = prior.latent_param_map(mesh_rep) if learned else prior.compute_dist_params(grid_emb)
+            mean, std = prior.mean_std(dist)
+            latent_emb = dec.latent_embedder.apply_rows([mean + eps * std])
+        mesh_rep = dec.mesh_step(grid_emb, latent_emb, ge)
+        return self._decode(mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+
+    def _decode(self, mesh_rep, grid_rep, m2g_emb, prev_state, boundary, bmask, out):
+        """m2g + param_map + (clamped) step epilogue with the boundary mix: the fused decoder where the graph / shapes allow,
+        else the launch chains ``BaseGraphModel.forward_with_boundary`` falls back to -> (new_state, pred_std|None)."""
+        dec = self.decoder
+        m2g, pm = dec.m2g_gnn, dec.param_map
+        clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
+        if clamp is None and not self.output_std:
+            fused = m2g.decode_step(mesh_rep, grid_rep, m2g_emb, pm, prev_state, boundary, bmask, self.diff_std, self.diff_mean,
+                                    out_flags=pm.nlam_flags, out=out)
+            if fused is not None:
+                return fused, None
+            aggr = m2g.aggregate_only(mesh_rep, grid_rep, m2g_emb)
+            if aggr is not None:
+                fused = ops.node_update_step(m2g.aggr_mlp, pm, grid_rep, aggr, prev_state, boundary, bmask, self.diff_std,
+                                             self.diff_mean, flags=pm.nlam_flags, out=out)
+                if fused is not None:
+                    return fused, None
+                grid_rep = m2g._kernel_node_update(grid_rep, aggr)
+            else:
+                grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
+            fused = ops.rowmlp_step(pm, grid_rep, prev_state, boundary, bmask, self.diff_std, self.diff_mean,
+                                    flags=pm.nlam_flags, out=out)
+            if fused is not None:
+                return fused, None
+        else:
+            grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
+        net_output = pm(grid_rep)
+        pred_std = None
+        if self.output_std:
+            net_output, std_raw = net_output.chunk(2, dim=-1)
+            pred_std = torch.nn.functional.softplus(std_raw)
+        return ops.step_epilogue(net_output.contiguous(), prev_state, boundary, bmask, self.diff_std, self.diff_mean, out=out,
+                                 clamp=clamp), pred_std
+
+
 MODELS = {"graph_lam": GraphLAM, "hi_lam": HiLAM, "hi_lam_parallel": HiLAMParallel}
 
 
@@ -591,6 +790,10 @@ class ARForecaster(nn.Module):
         G, d, f = p.num_grid_nodes, p.num_state_vars, p.grid_input_dim - 2 * p.num_state_vars - p.grid_static_features.shape[1]
         bufs = {"forcing": torch.zeros(batch_size, G, f, device=dev), "boundary": torch.zeros(batch_size, G, d, device=dev),
                 "state": [torch.zeros(batch_size, G, d, device=dev) for _ in range(3)]}
+        if getattr(p, "samples_latent", False):
+            # a predictor that samples: every captured step first refills this buffer from the default generator of the
+            # device, so each replay draws fresh noise and torch.cuda.manual_seed makes a sequence of replays reproducible
+            bufs["latent_noise"] = torch.zeros(batch_size, p.num_mesh_nodes, p.latent_dim, device=dev)
         p.static_embeddings()  # materialise the weight-only embeddings outside the graph
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -625,8 +828,13 @@ class ARForecaster(nn.Module):
 
     def _one_step(self, bufs, k):
         st = bufs["state"]
+        noise = bufs.get("latent_noise")
+        if noise is None:
+            return self.predictor.forward_with_boundary(st[(k + 1) % 3], st[k % 3], bufs["forcing"], bufs["boundary"],
+                                                        self.boundary_mask, out=st[(k + 2) % 3])
+        noise.normal_()
         return self.predictor.forward_with_boundary(st[(k + 1) % 3], st[k % 3], bufs["forcing"], bufs["boundary"],
-                                                    self.boundary_mask, out=st[(k + 2) % 3])
+                                                    self.boundary_mask, latent_noise=noise, out=st[(k + 2) % 3])
 
     def set_state(self, prev_prev_state, prev_state):
         """Load the two initial states into the captured step's state ring."""

@@ -518,12 +518,13 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
     return out
 
 
-def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=0):
+def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=0, want_emb=False):
     """The grid side of a forecast step's encoder in ONE launch (``nlam_encode_fwd``): ``grid_emb = embed_seq(cat sources)``
     stays on chip; returns ``(grid_rep, proj)`` with ``grid_rep = grid_emb + grid_seq(grid_emb)`` (B, G, 64) and
     ``proj = [P_s | P_r]`` flat, ``P_s = grid_emb·W1sᵀ`` (B, G, 64) and ``P_r = mesh·W1rᵀ + b1`` (n_mesh, 64) of the grid -> mesh
     layer's edge MLP ``edge_seq`` on ``graph`` — the ``proj_in`` of that layer's ``inet_fwd`` with send = P_s.  ``mesh`` and
-    ``edge_csr`` are shared by the batch.  Returns None when the library does not fuse these shapes / this math mode (the
+    ``edge_csr`` are shared by the batch.  ``want_emb``: also store grid_emb (``nlam_encode_emb_fwd``) and return
+    ``(grid_rep, proj, grid_emb)``.  Returns None when the library does not fuse these shapes / this math mode (the
     caller then runs the embedder, the g2m layer and ``grid_seq`` as three calls)."""
     L = _lib.lib()
     if flags & _lib.MATH_FP32:
@@ -547,14 +548,46 @@ def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=
     em, gm, sm = mlp_struct(embed_seq), mlp_struct(grid_seq), mlp_struct(edge_seq)
     grid_rep = torch.empty((B, G, 64), device=m.device, dtype=torch.float32)
     proj = torch.empty((B * G + graph.n_rec) * 64, device=m.device, dtype=torch.float32)
+    args = (m.data_ptr(), mbs if Bm > 1 else 0, e.data_ptr(), ebs if Be > 1 else 0, grid_rep.data_ptr(), proj.data_ptr())
+    grid_emb = torch.empty((B, G, 64), device=m.device, dtype=torch.float32) if want_emb else None
     with torch.cuda.device(m.device):
-        rc = L.nlam_encode_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
-                               m.data_ptr(), mbs if Bm > 1 else 0, e.data_ptr(), ebs if Be > 1 else 0, grid_rep.data_ptr(),
-                               proj.data_ptr(), G, B, flags, _stream_ptr(m.device))
+        if want_emb:
+            rc = L.nlam_encode_emb_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
+                                       *args, grid_emb.data_ptr(), G, B, flags, _stream_ptr(m.device))
+        else:
+            rc = L.nlam_encode_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
+                                   *args, G, B, flags, _stream_ptr(m.device))
     if rc == _lib.E_UNSUPPORTED:
         return None
     _lib.check(rc)
-    return grid_rep, proj
+    return (grid_rep, proj, grid_emb) if want_emb else (grid_rep, proj)
+
+
+def latent_sample(param_seq, embed_seq, x, eps, flags=0):
+    """Graph-EFM's latent step in ONE launch (``nlam_latent_sample_fwd``): ``p = param_seq(x)``, ``mean, std`` from p
+    (64 outputs: std = 1; 128 outputs: std = 1e-4 + softplus(p[..., 64:])), ``z = mean + eps * std`` and
+    ``embed_seq(z)`` -> (B, N, 64); p and z stay on chip.  ``x``, ``eps``: (B, N, 64).  Returns None when the library does not
+    fuse these shapes / this math mode (the caller then composes the three steps)."""
+    L = _lib.lib()
+    if flags & _lib.MATH_FP32:
+        return None
+    xr, Bx, xbs = as_rows(x)
+    er, Be, ebs = as_rows(eps)
+    _require_cuda(xr, er)
+    B = max(Bx, Be)
+    if (Bx not in (1, B) or Be not in (1, B) or xr.shape[-1] != 64 or er.shape[-1] != 64 or er.shape[-2] != xr.shape[-2]
+            or xr.device != er.device):
+        return None
+    pm, em = mlp_struct(param_seq), mlp_struct(embed_seq)
+    N = xr.shape[-2]
+    out = torch.empty((B, N, 64), device=xr.device, dtype=torch.float32)
+    args = (ctypes.byref(pm), ctypes.byref(em), xr.data_ptr(), xbs if Bx > 1 else 0, er.data_ptr(), ebs if Be > 1 else 0,
+            out.data_ptr(), N, B, flags)
+    if not L.nlam_latent_sample_supported(*args):
+        return None
+    with torch.cuda.device(xr.device):
+        _lib.check(L.nlam_latent_sample_fwd(*args, _stream_ptr(xr.device)))
+    return out
 
 
 class RecomputeFn(torch.autograd.Function):
