@@ -221,6 +221,20 @@ int nlam_encode_emb_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const Nl
                         const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge,
                         int64_t edge_bstride, float* grid_rep, float* proj, float* grid_emb, int64_t n_rows, int B, int flags,
                         void* stream);
+/* nlam_encode_fwd for two grid -> mesh layers on the same grid embedding, receivers and edge features (the hierarchical
+ * Graph-EFM's prior and decoder g2m layers, reference latent/hi_graph_encoder.py:148-150, hi_graph_decoder.py:216-218): the
+ * launch also computes proj_b = [P_s_b (B, n_rows, 64) | P_r_b (n_rec, 64)] of g2m_edge_mlp_b, the proj_in of the second
+ * layer's nlam_inet_fwd_chain call (send = P_s_b).  grid_emb is not stored.  Covered where nlam_encode_fwd covers the first
+ * layer and the second layer's call takes the same batch-broadcast split edge path; nlam_encode2_supported says whether a
+ * call is.  NLAM_E_UNSUPPORTED otherwise. */
+int nlam_encode2_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
+                           const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b, const float* mesh,
+                           int64_t mesh_bstride, const float* g2m_edge, int64_t edge_bstride, const float* grid_rep,
+                           const float* proj, const float* proj_b, int64_t n_rows, int B, int flags);
+int nlam_encode2_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
+                     const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b, const float* mesh, int64_t mesh_bstride,
+                     const float* g2m_edge, int64_t edge_bstride, float* grid_rep, float* proj, float* proj_b, int64_t n_rows,
+                     int B, int flags, void* stream);
 /* The stochastic step of Graph-EFM (reference latent/graph_encoder.py:102-105, base_encoder.py:85-94,
  * base_decoder.py:145) in one launch (csrc/fused.cu).  Per row r of batch element b, x (B, n_rows, 64) the prior's mesh
  * representation and eps (B, n_rows, 64) standard normal noise, both with dense rows and batch strides x_bstride /

@@ -120,7 +120,8 @@ bool tc_encode_supported(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n
                          const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags);
 int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp,
               const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags, float* grid_rep, float* ps, float* pr,
-              float* grid_emb, cudaStream_t st);
+              float* grid_emb, cudaStream_t st, const NlamMlp* g2m_edge_mlp_b = nullptr, float* ps_b = nullptr,
+              float* pr_b = nullptr);
 // fused.cu: Graph-EFM's latent step in one kernel: prior latent_param_map, reparameterised sample, decoder latent_embedder
 bool tc_latent_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs, const float* eps,
                          int64_t eps_bs, const float* out, int64_t n_rows, int B, int flags);

@@ -648,17 +648,25 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_
 // copied with cp.async into a raw fp32 staging buffer while the previous item's GEMMs run; a dense source's rows of one
 // item are one contiguous span, copied in 16-byte pieces where it starts 16-byte aligned and element by element otherwise.
 // EMIT_EMB: grid_emb is also stored (B, n_rows, 64): Graph-EFM's decoder reads it as the senders of its g2m layer.
+// TWO_G2M (tc_encode2_kernel): the projections of a second g2m edge MLP on the same grid_emb are computed as well,
+// P_s_b = grid_emb·W1s_bᵀ after P_s, and P_r_b = mesh·W1r_bᵀ + b1_b by a second set of mesh items: the hierarchical Graph-EFM's
+// prior and decoder g2m layers share their senders (grid_emb), receivers and edge features, so grid_emb never goes to HBM.
+// The weights go through fz_load_w and grid_emb through fz_store_op as for the first layer: both round to nearest.
 namespace enc {
 using fz::CH_A;
 using fz::CH_W;
 constexpr uint32_t WE1 = 0, WE2 = WE1 + 2 * CH_W, W1S = WE2 + 2 * CH_W, WA1 = W1S + 2 * CH_W, WA2 = WA1 + 2 * CH_W,
-                   W1R = WA2 + 2 * CH_W;
-constexpr uint32_t A = W1R + 2 * CH_W;    // 128 x 64 operand, 64 rows per warp group
-constexpr uint32_t STG = A + 2 * CH_A;    // per warp group: 64 rows x at most 64 columns of raw inputs, source by source
-constexpr uint32_t COLS = STG + 2 * 64 * 64 * 4;  // operand column c <- staging float cols[c].x + row * cols[c].y (y = 0: zero)
-constexpr uint32_t PRM = COLS + 64 * 8;   // be1, be2, gamma, beta (embedder) | ba1, ba2, gamma, beta (grid MLP) | b1 (g2m)
-constexpr uint32_t BYTES = PRM + 9 * 64 * 4 + 1024;  // + alignment slack
-static_assert(BYTES <= 227 * 1024, "encoder shared memory exceeds the sm_90 limit");
+                   W1R = WA2 + 2 * CH_W, W1S_B = W1R + 2 * CH_W, W1R_B = W1S_B + 2 * CH_W;  // W1S_B / W1R_B: TWO_G2M only
+template <bool TWO_G2M>
+struct Layout {
+  static constexpr uint32_t A = (TWO_G2M ? W1R_B : W1R) + 2 * CH_W;  // 128 x 64 operand, 64 rows per warp group
+  static constexpr uint32_t STG = A + 2 * CH_A;  // per warp group: 64 rows x at most 64 columns of raw inputs, source by source
+  static constexpr uint32_t COLS = STG + 2 * 64 * 64 * 4;  // operand column c <- staging float cols[c].x + row * cols[c].y (y = 0: zero)
+  // be1, be2, gamma, beta (embedder) | ba1, ba2, gamma, beta (grid MLP) | b1 (g2m) | b1_b (second g2m, TWO_G2M only)
+  static constexpr uint32_t PRM = COLS + 64 * 8;
+  static constexpr uint32_t BYTES = PRM + (TWO_G2M ? 10 : 9) * 64 * 4 + 1024;  // + alignment slack
+  static_assert(BYTES <= 227 * 1024, "encoder shared memory exceeds the sm_90 limit");
+};
 }  // namespace enc
 
 struct EncParams {
@@ -674,22 +682,26 @@ struct EncParams {
   const float* mesh;            // (n_mesh, 64), shared by the batch
   float* pr;                    // (n_mesh, 64)
   long long n_mesh, n_mesh_tiles;
+  FzW w1s_b, w1r_b;             // TWO_G2M only: the second g2m edge MLP
+  const float* b1_b;
+  float *ps_b, *pr_b;           // (B, n_rows, 64), (n_mesh, 64)
 };
 
-template <bool EMIT_EMB>
+template <bool EMIT_EMB, bool TWO_G2M>
 __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_constant__ EncParams p) {
   using namespace fz;
+  using Lay = enc::Layout<TWO_G2M>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const uint32_t sb = smem_u32(s);
-  uint8_t* sA = s + enc::A;
-  float* prm = reinterpret_cast<float*>(s + enc::PRM);
-  int2* cols = reinterpret_cast<int2*>(s + enc::COLS);
+  uint8_t* sA = s + Lay::A;
+  float* prm = reinterpret_cast<float*>(s + Lay::PRM);
+  int2* cols = reinterpret_cast<int2*>(s + Lay::COLS);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
   const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // operand row of fragment half 0 (half 1: + 8)
   const int lr = rq - 64 * wg;                              // the same row within the warp group's 64
-  const uint32_t aA = sb + enc::A + wg * (CH_A / 2);
-  float* stg = reinterpret_cast<float*>(s + enc::STG) + wg * 64 * 64;
+  const uint32_t aA = sb + Lay::A + wg * (CH_A / 2);
+  float* stg = reinterpret_cast<float*>(s + Lay::STG) + wg * 64 * 64;
   const uint32_t stg_u = smem_u32(stg);
 
   fz_load_w(s + enc::WE1, p.we1, 2, tid);
@@ -698,6 +710,10 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
   fz_load_w(s + enc::WA1, p.wa1, 2, tid);
   fz_load_w(s + enc::WA2, p.wa2, 2, tid);
   fz_load_w(s + enc::W1R, p.w1r, 2, tid);
+  if (TWO_G2M) {
+    fz_load_w(s + enc::W1S_B, p.w1s_b, 2, tid);
+    fz_load_w(s + enc::W1R_B, p.w1r_b, 2, tid);
+  }
   for (int i = tid; i < 64; i += THREADS) {
     prm[i] = p.be1[i];
     prm[64 + i] = p.be2[i];
@@ -708,6 +724,7 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
     prm[384 + i] = p.gamma_a[i];
     prm[448 + i] = p.beta_a[i];
     prm[512 + i] = p.b1[i];
+    if (TWO_G2M) prm[576 + i] = p.b1_b[i];
     int2 m = make_int2(0, 0);
     for (int q = 0, off = 0; q < p.n_src; off += p.src[q].dim, ++q)
       if (i >= off && i < off + p.src[q].dim) m = make_int2(64 * off + i - off, p.src[q].dim);
@@ -716,7 +733,7 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
   fence_proxy_async();
   __syncthreads();  // the last CTA-wide barrier: from here on each warp group runs on its own
 
-  const long long n_grid = p.n_tiles * p.B, n_items = n_grid + p.n_mesh_tiles;
+  const long long n_grid = p.n_tiles * p.B, n_items = n_grid + (TWO_G2M ? 2 : 1) * p.n_mesh_tiles;
   const long long stride = 2LL * gridDim.x;
   const uint64_t pol_stream = policy_evict_first(), pol_shared = policy_evict_normal();
   // the raw input rows of grid item it -> staging (source q at float 64 * (dim_0 + ... + dim_{q-1}), rows dense)
@@ -742,8 +759,10 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
   if (item < n_grid) issue(item);
   for (; item < n_items; item += stride) {
     if (item >= n_grid) {
-      // ---- P_r = mesh·W1rᵀ + b1 for 64 mesh rows (few items: loaded without staging)
-      const long long row0 = (item - n_grid) * 64;
+      // ---- P_r = mesh·W1rᵀ + b1 for 64 mesh rows (few items: loaded without staging); TWO_G2M: the items after the first
+      // n_mesh_tiles compute P_r_b
+      const bool second = TWO_G2M && item - n_grid >= p.n_mesh_tiles;
+      const long long row0 = (item - n_grid - (second ? p.n_mesh_tiles : 0)) * 64;
       float4 x[8];
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
@@ -756,12 +775,13 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
         *reinterpret_cast<float4*>(sA + fz_off(CH_A, 64 * wg + 8 * q + (gt >> 4), (gt & 15) * 4)) = tf32r4(x[q]);
       fence_proxy_async();
       named_bar_sync(bar, 128);
-      fz_gemm(acc, aA, sb + enc::W1R, 2);
-      fz_unpack(acc, v, prm + 512);
+      fz_gemm(acc, aA, sb + (second ? enc::W1R_B : enc::W1R), 2);
+      fz_unpack(acc, v, prm + (second ? 576 : 512));
       const long long r0 = row0 + lr;
+      float* pr = second ? p.pr_b : p.pr;
 #pragma unroll
       for (int i = 0; i < 2; ++i)
-        if (r0 + 8 * i < p.n_mesh) fz_store_row64(p.pr + (r0 + 8 * i) * 64, v[i]);
+        if (r0 + 8 * i < p.n_mesh) fz_store_row64(pr + (r0 + 8 * i) * 64, v[i]);
       continue;
     }
     const int b = (int)(item / p.n_tiles);
@@ -814,6 +834,12 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_encode_kernel(const __grid_
     fz_unpack(acc, v, nullptr);
     if (valid0) fz_store_row64(p.ps + o, v[0]);
     if (valid1) fz_store_row64(p.ps + o + 8 * 64, v[1]);
+    if (TWO_G2M) {  // ---- 3b. P_s_b = grid_emb·W1s_bᵀ, on the same operand
+      fz_gemm(acc, aA, sb + enc::W1S_B, 2);
+      fz_unpack(acc, v, nullptr);
+      if (valid0) fz_store_row64(p.ps_b + o, v[0]);
+      if (valid1) fz_store_row64(p.ps_b + o + 8 * 64, v[1]);
+    }
     // ---- 4. grid_rep = grid_emb + encoding grid MLP(grid_emb)
     fz_gemm(acc, aA, sb + enc::WA1, 2);
     fz_unpack(acc, v, prm + 256);
@@ -1486,11 +1512,16 @@ bool tc_encode_supported(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n
 
 int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp,
               const float* mesh, int64_t n_mesh, int64_t n_rows, int B, int flags, float* grid_rep, float* ps, float* pr,
-              float* grid_emb, cudaStream_t st) {
+              float* grid_emb, cudaStream_t st, const NlamMlp* g2m_edge_mlp_b, float* ps_b, float* pr_b) {
   NLAM_REQUIRE(tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, n_mesh, n_rows, B, flags),
                NLAM_E_UNSUPPORTED, "tc_encode: unsupported shapes");
-  NLAM_REQUIRE(aligned16(grid_rep) && aligned16(ps) && aligned16(pr) && aligned16(grid_emb), NLAM_E_INVALID,
-               "tc_encode: unaligned outputs");
+  const bool two = g2m_edge_mlp_b != nullptr;
+  NLAM_REQUIRE(!two || (enc_mlp_ok(g2m_edge_mlp_b, 192) && g2m_edge_mlp_b->in_dim == 192), NLAM_E_UNSUPPORTED,
+               "tc_encode: unsupported second g2m edge MLP");
+  NLAM_REQUIRE(!(two && grid_emb), NLAM_E_INVALID, "tc_encode: grid_emb is not stored with a second g2m edge MLP");
+  NLAM_REQUIRE(aligned16(grid_rep) && aligned16(ps) && aligned16(pr) && aligned16(grid_emb) && aligned16(ps_b) &&
+                   aligned16(pr_b) && (!two || (ps_b && pr_b)),
+               NLAM_E_INVALID, "tc_encode: unaligned or missing outputs");
   EncParams p;
   memset(&p, 0, sizeof(p));
   p.B = B;
@@ -1526,26 +1557,39 @@ int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const
   p.pr = pr;
   p.n_mesh = n_mesh;
   p.n_mesh_tiles = (n_mesh + 63) / 64;
-  const long long n_items = p.n_tiles * B + p.n_mesh_tiles;
+  if (two) {
+    p.w1s_b = wslice(g2m_edge_mlp_b->w[0] + 64, 192, 64, 64);
+    p.w1r_b = wslice(g2m_edge_mlp_b->w[0] + 128, 192, 64, 64);
+    p.b1_b = g2m_edge_mlp_b->b[0];
+    p.ps_b = ps_b;
+    p.pr_b = pr_b;
+  }
+  const long long n_items = p.n_tiles * B + (two ? 2 : 1) * p.n_mesh_tiles;
   NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_encode: bad work size");
   int dev = 0;
   NLAM_CUDA_OK(cudaGetDevice(&dev));
   static unsigned mask = 0;
   if (!(mask & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc::BYTES));
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc::BYTES));
+    const int b1 = (int)enc::Layout<false>::BYTES, b2 = (int)enc::Layout<true>::BYTES;
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b1));
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b1));
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2));
     mask |= 1u << (dev & 31);
   }
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
-  // algorithmic bytes: the inputs once, grid_rep and P_s (and grid_emb), the mesh rows and P_r, the weights
-  bytes += (grid_emb ? 3.0 : 2.0) * 4.0 * 64 * n_rows * B + 2.0 * 4.0 * 64 * n_mesh +
-           4.0 * (embed_mlp->in_dim * 64 + 5 * 64 * 64 + 9 * 64);
-  {
+  // algorithmic bytes: the inputs once, grid_rep and P_s (and grid_emb or P_s_b), the mesh rows and P_r (and P_r_b), the
+  // weights
+  bytes += ((grid_emb || two) ? 3.0 : 2.0) * 4.0 * 64 * n_rows * B + (two ? 3.0 : 2.0) * 4.0 * 64 * n_mesh +
+           4.0 * (embed_mlp->in_dim * 64 + (two ? 7 : 5) * 64 * 64 + (two ? 10 : 9) * 64);
+  if (two) {
+    ProfScope ps_("tc_encode2_kernel", st, bytes);
+    tc_encode_kernel<false, true><<<grid, fz::THREADS, enc::Layout<true>::BYTES, st>>>(p);
+  } else {
     ProfScope ps_("tc_encode_kernel", st, bytes);
     if (grid_emb)
-      tc_encode_kernel<true><<<grid, fz::THREADS, enc::BYTES, st>>>(p);
+      tc_encode_kernel<true, false><<<grid, fz::THREADS, enc::Layout<false>::BYTES, st>>>(p);
     else
-      tc_encode_kernel<false><<<grid, fz::THREADS, enc::BYTES, st>>>(p);
+      tc_encode_kernel<false, false><<<grid, fz::THREADS, enc::Layout<false>::BYTES, st>>>(p);
   }
   count_launch();
   NLAM_CUDA_OK(cudaGetLastError());

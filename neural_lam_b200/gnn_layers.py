@@ -339,11 +339,12 @@ class InteractionNet(nn.Module):
         return self._halo is None and self.update_edges and self._fusable() and self._is_sorted and not self.propagation
 
     @torch.no_grad()
-    def forward_stacked(self, node_rep, edge_rep, first, last, proj_in=None, next_layer=None):
+    def forward_stacked(self, node_rep, edge_rep, first, last, proj_in=None, next_layer=None, keep_edges=False):
         """Inference-only entry for a layer inside a stack over ONE node set whose intermediate edge tensors are
         private to the stack (``GNNSequential`` with ``keep_edge_rep=False``): the last layer does not write its
         edge output (nobody reads it), a middle layer may update ``edge_rep`` in place (``first``: the incoming
-        tensor belongs to the caller — e.g. the cached static embedding — and is never written).  Same values as
+        tensor belongs to the caller — e.g. the cached static embedding — and is never written).  ``keep_edges``: the last
+        layer writes its edge output too, in place like a middle layer unless it is also the first.  Same values as
         ``forward``.  ``proj_in``: this layer's node projections, computed by the previous layer's node kernel;
         ``next_layer``: the following layer of the stack — when the library supports it for both, this call's node kernel
         also computes that layer's projections (csrc/fused.cu).  Returns ``(node_rep', edge_rep' | None, proj_next | None)``."""
@@ -353,7 +354,8 @@ class InteractionNet(nn.Module):
         self._check_inputs(node_rep, node_rep, edge_rep)
         _, (s3, r3, e3) = self._batchify(node_rep, node_rep, edge_rep)
         g = self._graph(r3.device)
-        inplace = _INPLACE_EDGE_UPDATE and (not first) and (not last) and e3.is_contiguous()
+        write_edges = keep_edges or not last
+        inplace = _INPLACE_EDGE_UPDATE and (not first) and write_edges and e3.is_contiguous()
         nxt = None
         if (_CHAIN_PROJECTIONS and next_layer is not None and isinstance(next_layer, InteractionNet) and next_layer._stackable()
                 and self._stackable() and next_layer.num_rec == self.num_rec and r3.shape[0] > 0):
@@ -363,10 +365,10 @@ class InteractionNet(nn.Module):
                                                  next_layer._flags())):
                 nxt = next_layer.edge_mlp
         if proj_in is None and nxt is None:
-            rec_out, edge_out, _ = ops.inet_fwd(g, self.edge_mlp, self.aggr_mlp, s3, r3, e3, not last, self._flags(),
+            rec_out, edge_out, _ = ops.inet_fwd(g, self.edge_mlp, self.aggr_mlp, s3, r3, e3, write_edges, self._flags(),
                                                 edge_inplace=inplace)
             return rec_out, edge_out, None
-        rec_out, edge_out, _, proj_out = ops.inet_fwd(g, self.edge_mlp, self.aggr_mlp, s3, r3, e3, not last, self._flags(),
+        rec_out, edge_out, _, proj_out = ops.inet_fwd(g, self.edge_mlp, self.aggr_mlp, s3, r3, e3, write_edges, self._flags(),
                                                       edge_inplace=inplace, proj_in=proj_in, next_edge_seq=nxt)
         return rec_out, edge_out, proj_out
 
@@ -391,28 +393,53 @@ class InteractionNet(nn.Module):
                                diff_std, diff_mean, flags=self._flags() | out_flags, out=out)
 
     @torch.no_grad()
-    def encode_step(self, embedder, grid_mlp, grid_inputs, rec_rep, edge_rep, want_grid_emb=False):
+    def encode_step(self, embedder, grid_mlp, grid_inputs, rec_rep, edge_rep, want_grid_emb=False, second=None):
         """Inference-only, for the grid -> mesh layer of a forecast step: ``grid_emb = embedder(cat grid_inputs)``, this layer's
         node projections and ``grid_rep = grid_emb + grid_mlp(grid_emb)`` in one launch (``ops.encode``; grid_emb never goes
         to HBM), then this layer's edge stage on those projections and its node update.  Returns ``(rec_rep', grid_rep)``, or
         None when the layer / graph / call shape has no such path (the caller then runs the three calls).
-        ``want_grid_emb``: the launch also stores grid_emb, returned third (Graph-EFM's decoder reads it)."""
+        ``want_grid_emb``: the launch also stores grid_emb, returned third (Graph-EFM's decoder reads it).
+        ``second``: another grid -> mesh layer on the same graph, receivers and edge features, with grid_emb as its senders
+        (the hierarchical Graph-EFM's decoder g2m): the launch also computes its projections, and its output is returned
+        third; grid_emb is not stored."""
         if not self._edge_stage_separable():
+            return None
+        if second is not None and not (second._edge_stage_separable() and self._same_edges(second)):
             return None
         _, (r3, e3) = self._batchify(rec_rep, edge_rep)
         if r3.shape[-2] != self.num_rec or e3.shape[-2] != self.num_edges or r3.device != self._src32.device:
             return None
         g = self._graph(r3.device)
         fl = self._flags() | embedder.nlam_flags | grid_mlp.nlam_flags
-        enc = ops.encode(g, embedder, grid_inputs, grid_mlp, self.edge_mlp, r3, e3, flags=fl, want_emb=want_grid_emb)
+        if second is not None:
+            fl |= second._flags()
+        enc = ops.encode(g, embedder, grid_inputs, grid_mlp, self.edge_mlp, r3, e3, flags=fl, want_emb=want_grid_emb,
+                         edge_seq_b=second.edge_mlp if second is not None else None)
         if enc is None:
             return None
-        grid_rep, proj = enc[:2]
+        grid_rep = enc[0]
         B, G = grid_rep.shape[0], grid_rep.shape[1]
-        ps = proj[: B * G * 64].view(B, G, 64)
-        rec_out, _, _, _ = ops.inet_fwd(g, self.edge_mlp, self.aggr_mlp, ps, r3.expand(B, -1, -1), e3.expand(B, -1, -1), False,
-                                        self._flags(), proj_in=proj)
-        return (rec_out, grid_rep, enc[2]) if want_grid_emb else (rec_out, grid_rep)
+        outs = []
+        for layer, proj in ((self, enc[1]), (second, enc[2] if second is not None else None)):
+            if layer is None:
+                continue
+            ps = proj[: B * G * 64].view(B, G, 64)
+            rec_out, _, _, _ = ops.inet_fwd(layer._graph(r3.device), layer.edge_mlp, layer.aggr_mlp, ps, r3.expand(B, -1, -1),
+                                            e3.expand(B, -1, -1), False, layer._flags(), proj_in=proj)
+            outs.append(rec_out)
+        if second is not None:
+            return outs[0], grid_rep, outs[1]
+        return (outs[0], grid_rep, enc[2]) if want_grid_emb else (outs[0], grid_rep)
+
+    def _same_edges(self, other):
+        """Does ``other`` have this layer's edge set?  Compared once per pair (outside any CUDA-graph capture: the first
+        no-grad step runs eagerly)."""
+        memo = self.__dict__.setdefault("_same_edges_memo", {})
+        key = (id(other), other.edge_index.data_ptr(), self.edge_index.data_ptr())
+        if key not in memo:
+            memo[key] = (other.num_rec == self.num_rec and other.num_edges == self.num_edges
+                         and torch.equal(other.edge_index.cpu(), self.edge_index.cpu()))
+        return memo[key]
 
     @torch.no_grad()
     def aggregate_only(self, send_rep, rec_rep, edge_rep):

@@ -25,7 +25,8 @@ from torch import nn
 from . import _lib, ops
 from .gnn_layers import InteractionNet, get_gnn_class
 from . import clamping
-from .latent import ConstantLatentEncoder, GraphLatentDecoder, GraphLatentEncoder
+from .latent import (ConstantLatentEncoder, GraphLatentDecoder, GraphLatentEncoder, HiGraphLatentDecoder,
+                     HiGraphLatentEncoder)
 from .clamping import OutputClamp
 from .networks import GNNSequential, make_mlp
 from .synthetic import normalize_graph
@@ -510,26 +511,25 @@ class HiLAMParallel(BaseHiGraphModel):
         return levels, list(sections[:L]), list(sections[L:2 * L - 1]), list(sections[2 * L - 1:])
 
 
-class GraphEFMMultiScale(BaseGraphModel):
-    """Graph-EFM, the latent-variable ensemble forecaster, on a flat (multiscale) mesh (reference
-    step_predictors/graph/graph_efm.py: BaseGraphEFM :25-471, GraphEFMMultiScale :796-1037).  ``forward`` samples one step
-    from the prior: grid embedding, prior over a latent on the mesh nodes, reparameterised sample, decoder.  The
-    variational posterior is ``self.encoder`` (conditioned on the target through ``embedd_grid_with_target``); the
-    predictor computes no loss.
+class BaseGraphEFM(BaseGraphModel):
+    """Graph-EFM, the latent-variable ensemble forecaster (reference step_predictors/graph/graph_efm.py: BaseGraphEFM
+    :25-471).  ``forward`` samples one step from the prior: grid embedding, prior over a latent on mesh nodes,
+    reparameterised sample, decoder.  The variational posterior is ``self.encoder`` (conditioned on the target through
+    ``embedd_grid_with_target``); the predictor computes no loss.
 
     Submodule names and persistent buffers are the reference's, so its state_dicts load strictly.  The graph registration
     and the cache of the weight-only embeddings are ``BaseGraphModel``'s; the encode-process-decode modules of
-    ``BaseGraphModel.__init__`` are not built (``StepPredictor.__init__`` runs instead).
+    ``BaseGraphModel.__init__`` are not built (``StepPredictor.__init__`` runs instead).  Subclasses define the mesh: its
+    graph type, ``latent_spatial_dim``, the learnable prior, the weight-only embeddings and the no-grad ``_step``.
 
-    Noise: ``latent_noise`` (B, N_mesh, latent_dim) is the standard normal ε of ``z = mean + ε * std``; without it ε is
-    drawn with ``torch.randn`` on the default generator of the current device.  Under autograd the sample is composed from
-    the module outputs in that order; the no-grad step runs the fused kernels where they cover the shapes."""
+    Noise: ``latent_noise`` (B, latent_spatial_dim, latent_dim) is the standard normal ε of ``z = mean + ε * std``; without
+    it ε is drawn with ``torch.randn`` on the default generator of the current device.  Under autograd the sample is
+    composed from the module outputs in that order; the no-grad step runs the fused kernels where they cover the shapes."""
 
     samples_latent = True
 
-    def __init__(self, datastore, graph, hidden_dim=64, hidden_layers=1, latent_dim=None, prior_m2m_layers=2,
-                 encoder_m2m_layers=2, decoder_m2m_layers=4, learn_prior=True, prior_dist="isotropic",
-                 g2m_gnn_type="InteractionNet", m2g_gnn_type="InteractionNet", output_std=False,
+    def __init__(self, datastore, graph, hidden_dim=64, hidden_layers=1, latent_dim=None, prior_layers=2, learn_prior=True,
+                 prior_dist="isotropic", g2m_gnn_type="InteractionNet", m2g_gnn_type="InteractionNet", output_std=False,
                  output_clamping_lower=None, output_clamping_upper=None, math=None):
         StepPredictor.__init__(self, datastore, output_std=output_std, output_clamping_lower=output_clamping_lower,
                                output_clamping_upper=output_clamping_upper)
@@ -539,8 +539,7 @@ class GraphEFMMultiScale(BaseGraphModel):
         self.hidden_dim, self.hidden_layers, self.math = hidden_dim, hidden_layers, math
         g = graph if graph.get("normalized") else normalize_graph(graph)
         self.hierarchical = bool(g["hierarchical"])
-        if self.hierarchical:
-            raise ValueError(f"{type(self).__name__} requires a flat mesh graph, but the graph is hierarchical")
+        self.check_graph_type()
         self._register_graph(g)
         self.num_mesh_nodes, _ = self.get_num_mesh()
         self.grid_input_dim = self.grid_dim = datastore.grid_input_dim
@@ -553,54 +552,30 @@ class GraphEFMMultiScale(BaseGraphModel):
         self.m2g_embedder = make_mlp([m2g_dim] + self.mlp_blueprint_end)
         self.latent_dim = latent_dim if latent_dim is not None else hidden_dim
         if learn_prior:
-            self.prior_model = GraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, hidden_dim,
-                                                  prior_m2m_layers, hidden_layers=hidden_layers, g2m_gnn_type=g2m_gnn_type,
-                                                  output_dist=prior_dist, math=math)
+            self.prior_model = self.build_learnable_prior(prior_layers, prior_dist)
         else:
-            self.prior_model = ConstantLatentEncoder(self.latent_dim, self.num_mesh_nodes, output_dist=prior_dist)
-        self.mesh_embedder = make_mlp([self.mesh_static_features.shape[1]] + self.mlp_blueprint_end)
-        self.m2m_embedder = make_mlp([self.m2m_features.shape[1]] + self.mlp_blueprint_end)
-        self.encoder = GraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, hidden_dim,
-                                          encoder_m2m_layers, hidden_layers=hidden_layers, g2m_gnn_type=g2m_gnn_type,
-                                          output_dist="diagonal", math=math)
-        self.decoder = GraphLatentDecoder(self.g2m_edge_index, self.m2m_edge_index, self.m2g_edge_index, hidden_dim,
-                                          self.latent_dim, self.num_state_vars, decoder_m2m_layers, hidden_layers=hidden_layers,
-                                          g2m_gnn_type=g2m_gnn_type, m2g_gnn_type=m2g_gnn_type, output_std=bool(output_std),
-                                          math=math)
+            self.prior_model = ConstantLatentEncoder(self.latent_dim, self.latent_spatial_dim, output_dist=prior_dist)
         self._static_cache = None
-        self._set_mlp_flags()
 
-    def get_num_mesh(self):
-        return self.mesh_static_features.shape[0], 0
+    def check_graph_type(self):
+        raise NotImplementedError
 
     @property
     def latent_spatial_dim(self):
-        return self.num_mesh_nodes
+        raise NotImplementedError
 
-    def _static_params(self):
-        return [p for m in (self.g2m_embedder, self.m2g_embedder, self.mesh_embedder, self.m2m_embedder)
-                for p in m.parameters()]
-
-    def _compute_static(self):
-        return {"g2m_emb": self.g2m_embedder(self.g2m_features), "m2g_emb": self.m2g_embedder(self.m2g_features),
-                "mesh_emb": self.mesh_embedder(self.mesh_static_features),
-                "m2m_emb": self.m2m_embedder(self.m2m_features)}
+    def build_learnable_prior(self, prior_layers, prior_dist):
+        raise NotImplementedError
 
     def _graph_emb(self, batch_size):
-        st = self.static_embeddings()
-        return {k: self.expand_to_batch(st[f"{k}_emb"], batch_size) for k in ("g2m", "m2g", "mesh", "m2m")}
+        raise NotImplementedError
 
     def _grid_sources(self, prev_state, prev_prev_state, forcing):
         # Graph-EFM's order puts X_{t-1} first (graph_efm.py:386-394; GraphLAM puts X_t first)
         return [prev_prev_state, prev_state, forcing, self.expand_to_batch(self.grid_static_features, prev_state.shape[0])]
 
-    def embedd_mesh(self, batch_size):
-        """``mesh`` and ``m2m`` embeddings expanded to the batch (graph_efm.py:1015-1037)."""
-        ge = self._graph_emb(batch_size)
-        return {"mesh": ge["mesh"], "m2m": ge["m2m"]}
-
     def embedd_grid_and_graph(self, prev_state, prev_prev_state, forcing):
-        """-> (grid_emb (B, G, H), graph_emb {g2m, m2g, mesh, m2m}) (graph_efm.py:364-413)"""
+        """-> (grid_emb (B, G, H), graph_emb {g2m, m2g, mesh embeddings}) (graph_efm.py:364-413)"""
         grid_emb = self.grid_prev_embedder.apply_rows(self._grid_sources(prev_state, prev_prev_state, forcing))
         return grid_emb, self._graph_emb(prev_state.shape[0])
 
@@ -611,7 +586,7 @@ class GraphEFMMultiScale(BaseGraphModel):
         return self.grid_current_embedder.apply_rows([prev_prev, prev, forc, torch.cat((static, current_state), dim=-1)])
 
     def _noise(self, latent_noise, batch_size, device):
-        shape = (batch_size, self.num_mesh_nodes, self.latent_dim)
+        shape = (batch_size, self.latent_spatial_dim, self.latent_dim)
         if latent_noise is None:
             return torch.randn(shape, device=device)
         if tuple(latent_noise.shape) != shape:
@@ -639,39 +614,21 @@ class GraphEFMMultiScale(BaseGraphModel):
         assert not self.output_std
         return self._step(prev_state, prev_prev_state, forcing, latent_noise, boundary_state, boundary_mask, out)[0]
 
-    @torch.no_grad()
     def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
-        """The no-grad step: (1) grid embedder, decoder grid MLP and the prior g2m's projections in one launch, (2) prior g2m,
-        (3) prior m2m stack, (4) prior parameters + sample + latent embedding in one launch, (5) decoder g2m, (6) decoder
-        m2m stack, (7) m2g + param_map + step epilogue.  Each fused launch falls back to its composition where the library
-        does not cover the shapes."""
-        B = prev_state.shape[0]
-        ge = self._graph_emb(B)
+        raise NotImplementedError
+
+    def _sample_latent(self, mesh_rep, grid_emb, eps):
+        """Prior parameters + sample + latent embedding: one launch where the library covers the shapes, else composed.
+        ``mesh_rep``: the learned prior's representation on the latent's mesh nodes (None for a constant prior)."""
         prior, dec = self.prior_model, self.decoder
-        learned = isinstance(prior, GraphLatentEncoder)
-        sources = self._grid_sources(prev_state, prev_prev_state, forcing)
-        enc = None
-        if learned:
-            enc = prior.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, ge["mesh"], ge["g2m"],
-                                            want_grid_emb=True)
-        if enc is not None:
-            mesh_rep, res_grid, grid_emb = enc
-        else:
-            grid_emb = self.grid_prev_embedder.apply_rows(sources)
-            res_grid = dec.grid_update_mlp.apply_rows([grid_emb], res=grid_emb)
-            mesh_rep = prior.g2m_gnn(grid_emb, ge["mesh"], ge["g2m"]) if learned else None
-        eps = self._noise(latent_noise, B, prev_state.device)
-        latent_emb = None
-        if learned:
-            mesh_rep = prior.process_mesh(mesh_rep, ge["m2m"])
+        if mesh_rep is not None:
             latent_emb = ops.latent_sample(prior.latent_param_map, dec.latent_embedder, mesh_rep, eps,
                                            flags=prior.latent_param_map.nlam_flags | dec.latent_embedder.nlam_flags)
-        if latent_emb is None:
-            dist = prior.latent_param_map(mesh_rep) if learned else prior.compute_dist_params(grid_emb)
-            mean, std = prior.mean_std(dist)
-            latent_emb = dec.latent_embedder.apply_rows([mean + eps * std])
-        mesh_rep = dec.mesh_step(grid_emb, latent_emb, ge)
-        return self._decode(mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+            if latent_emb is not None:
+                return latent_emb
+        dist = prior.latent_param_map(mesh_rep) if mesh_rep is not None else prior.compute_dist_params(grid_emb)
+        mean, std = prior.mean_std(dist)
+        return dec.latent_embedder.apply_rows([mean + eps * std])
 
     def _decode(self, mesh_rep, grid_rep, m2g_emb, prev_state, boundary, bmask, out):
         """m2g + param_map + (clamped) step epilogue with the boundary mix: the fused decoder where the graph / shapes allow,
@@ -706,6 +663,211 @@ class GraphEFMMultiScale(BaseGraphModel):
             pred_std = torch.nn.functional.softplus(std_raw)
         return ops.step_epilogue(net_output.contiguous(), prev_state, boundary, bmask, self.diff_std, self.diff_mean, out=out,
                                  clamp=clamp), pred_std
+
+
+class GraphEFMMultiScale(BaseGraphEFM):
+    """Graph-EFM on a flat (multiscale) mesh (reference step_predictors/graph/graph_efm.py: GraphEFMMultiScale :796-1037):
+    the latent lives on every mesh node; prior and variational posterior are ``GraphLatentEncoder``s, the decoder is a
+    ``GraphLatentDecoder``."""
+
+    def __init__(self, datastore, graph, hidden_dim=64, hidden_layers=1, latent_dim=None, prior_m2m_layers=2,
+                 encoder_m2m_layers=2, decoder_m2m_layers=4, learn_prior=True, prior_dist="isotropic",
+                 g2m_gnn_type="InteractionNet", m2g_gnn_type="InteractionNet", output_std=False,
+                 output_clamping_lower=None, output_clamping_upper=None, math=None):
+        super().__init__(datastore, graph, hidden_dim=hidden_dim, hidden_layers=hidden_layers, latent_dim=latent_dim,
+                         prior_layers=prior_m2m_layers, learn_prior=learn_prior, prior_dist=prior_dist,
+                         g2m_gnn_type=g2m_gnn_type, m2g_gnn_type=m2g_gnn_type, output_std=output_std,
+                         output_clamping_lower=output_clamping_lower, output_clamping_upper=output_clamping_upper, math=math)
+        self.mesh_embedder = make_mlp([self.mesh_static_features.shape[1]] + self.mlp_blueprint_end)
+        self.m2m_embedder = make_mlp([self.m2m_features.shape[1]] + self.mlp_blueprint_end)
+        self.encoder = GraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, hidden_dim,
+                                          encoder_m2m_layers, hidden_layers=hidden_layers, g2m_gnn_type=g2m_gnn_type,
+                                          output_dist="diagonal", math=math)
+        self.decoder = GraphLatentDecoder(self.g2m_edge_index, self.m2m_edge_index, self.m2g_edge_index, hidden_dim,
+                                          self.latent_dim, self.num_state_vars, decoder_m2m_layers, hidden_layers=hidden_layers,
+                                          g2m_gnn_type=g2m_gnn_type, m2g_gnn_type=m2g_gnn_type, output_std=bool(output_std),
+                                          math=math)
+        self._set_mlp_flags()
+
+    def check_graph_type(self):
+        if self.hierarchical:
+            raise ValueError(f"{type(self).__name__} requires a flat mesh graph, but the graph is hierarchical")
+
+    def build_learnable_prior(self, prior_layers, prior_dist):
+        return GraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, self.hidden_dim, prior_layers,
+                                  hidden_layers=self.hidden_layers, g2m_gnn_type=self.g2m_gnn_type, output_dist=prior_dist,
+                                  math=self.math)
+
+    def get_num_mesh(self):
+        return self.mesh_static_features.shape[0], 0
+
+    @property
+    def latent_spatial_dim(self):
+        return self.num_mesh_nodes
+
+    def _static_params(self):
+        return [p for m in (self.g2m_embedder, self.m2g_embedder, self.mesh_embedder, self.m2m_embedder)
+                for p in m.parameters()]
+
+    def _compute_static(self):
+        return {"g2m_emb": self.g2m_embedder(self.g2m_features), "m2g_emb": self.m2g_embedder(self.m2g_features),
+                "mesh_emb": self.mesh_embedder(self.mesh_static_features),
+                "m2m_emb": self.m2m_embedder(self.m2m_features)}
+
+    def _graph_emb(self, batch_size):
+        st = self.static_embeddings()
+        return {k: self.expand_to_batch(st[f"{k}_emb"], batch_size) for k in ("g2m", "m2g", "mesh", "m2m")}
+
+    def embedd_mesh(self, batch_size):
+        """``mesh`` and ``m2m`` embeddings expanded to the batch (graph_efm.py:1015-1037)."""
+        ge = self._graph_emb(batch_size)
+        return {"mesh": ge["mesh"], "m2m": ge["m2m"]}
+
+    @torch.no_grad()
+    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
+        """The no-grad step: (1) grid embedder, decoder grid MLP and the prior g2m's projections in one launch, (2) prior g2m,
+        (3) prior m2m stack, (4) prior parameters + sample + latent embedding in one launch, (5) decoder g2m, (6) decoder
+        m2m stack, (7) m2g + param_map + step epilogue.  Each fused launch falls back to its composition where the library
+        does not cover the shapes."""
+        B = prev_state.shape[0]
+        ge = self._graph_emb(B)
+        prior, dec = self.prior_model, self.decoder
+        learned = isinstance(prior, GraphLatentEncoder)
+        sources = self._grid_sources(prev_state, prev_prev_state, forcing)
+        enc = None
+        if learned:
+            enc = prior.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, ge["mesh"], ge["g2m"],
+                                            want_grid_emb=True)
+        if enc is not None:
+            mesh_rep, res_grid, grid_emb = enc
+        else:
+            grid_emb = self.grid_prev_embedder.apply_rows(sources)
+            res_grid = dec.grid_update_mlp.apply_rows([grid_emb], res=grid_emb)
+            mesh_rep = prior.g2m_gnn(grid_emb, ge["mesh"], ge["g2m"]) if learned else None
+        eps = self._noise(latent_noise, B, prev_state.device)
+        if learned:
+            mesh_rep = prior.process_mesh(mesh_rep, ge["m2m"])
+        latent_emb = self._sample_latent(mesh_rep, grid_emb, eps)
+        mesh_rep = dec.mesh_step(grid_emb, latent_emb, ge)
+        return self._decode(mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+
+
+class GraphEFM(BaseGraphEFM):
+    """Graph-EFM on a hierarchical mesh, the reference's default Graph-EFM (reference step_predictors/graph/graph_efm.py:
+    GraphEFM :474-793): the latent lives on the top mesh level; prior and variational posterior are
+    ``HiGraphLatentEncoder``s, the decoder is a ``HiGraphLatentDecoder``.  ``m2m_embedders`` exist only when some stack has
+    intra-level layers (``embedd_m2m``)."""
+
+    def __init__(self, datastore, graph, hidden_dim=64, hidden_layers=1, latent_dim=None, prior_intra_level_layers=2,
+                 encoder_intra_level_layers=2, decoder_intra_level_layers=4, learn_prior=True, prior_dist="isotropic",
+                 g2m_gnn_type="InteractionNet", m2g_gnn_type="InteractionNet", output_std=False,
+                 output_clamping_lower=None, output_clamping_upper=None, math=None):
+        super().__init__(datastore, graph, hidden_dim=hidden_dim, hidden_layers=hidden_layers, latent_dim=latent_dim,
+                         prior_layers=prior_intra_level_layers, learn_prior=learn_prior, prior_dist=prior_dist,
+                         g2m_gnn_type=g2m_gnn_type, m2g_gnn_type=m2g_gnn_type, output_std=output_std,
+                         output_clamping_lower=output_clamping_lower, output_clamping_upper=output_clamping_upper, math=math)
+        self.num_levels = len(self.mesh_static_features)
+        self.level_mesh_sizes = [m.shape[0] for m in self.mesh_static_features]
+        L, end = self.num_levels, self.mlp_blueprint_end
+        mesh_dim = self.mesh_static_features[0].shape[1]
+        m2m_dim = self.m2m_features[0].shape[1]
+        up_dim, down_dim = self.mesh_up_features[0].shape[1], self.mesh_down_features[0].shape[1]
+        self.mesh_embedders = nn.ModuleList([make_mlp([mesh_dim] + end) for _ in range(L)])
+        self.mesh_up_embedders = nn.ModuleList([make_mlp([up_dim] + end) for _ in range(L - 1)])
+        self.mesh_down_embedders = nn.ModuleList([make_mlp([down_dim] + end) for _ in range(L - 1)])
+        self.embedd_m2m = max(prior_intra_level_layers, encoder_intra_level_layers, decoder_intra_level_layers) > 0
+        if self.embedd_m2m:
+            self.m2m_embedders = nn.ModuleList([make_mlp([m2m_dim] + end) for _ in range(L)])
+        self.encoder = HiGraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, self.mesh_up_edge_index,
+                                            hidden_dim, encoder_intra_level_layers, hidden_layers=hidden_layers,
+                                            g2m_gnn_type=g2m_gnn_type, output_dist="diagonal", math=math)
+        self.decoder = HiGraphLatentDecoder(self.g2m_edge_index, self.m2m_edge_index, self.m2g_edge_index,
+                                            self.mesh_up_edge_index, self.mesh_down_edge_index, hidden_dim, self.latent_dim,
+                                            self.num_state_vars, decoder_intra_level_layers, hidden_layers=hidden_layers,
+                                            g2m_gnn_type=g2m_gnn_type, m2g_gnn_type=m2g_gnn_type, output_std=bool(output_std),
+                                            math=math)
+        self._set_mlp_flags()
+
+    def check_graph_type(self):
+        if not self.hierarchical:
+            raise ValueError(f"{type(self).__name__} requires a hierarchical mesh graph, but the graph is flat")
+
+    def build_learnable_prior(self, prior_layers, prior_dist):
+        return HiGraphLatentEncoder(self.latent_dim, self.g2m_edge_index, self.m2m_edge_index, self.mesh_up_edge_index,
+                                    self.hidden_dim, prior_layers, hidden_layers=self.hidden_layers,
+                                    g2m_gnn_type=self.g2m_gnn_type, output_dist=prior_dist, math=self.math)
+
+    def get_num_mesh(self):
+        n = sum(m.shape[0] for m in self.mesh_static_features)
+        return n, n - self.mesh_static_features[0].shape[0]
+
+    @property
+    def latent_spatial_dim(self):
+        return self.mesh_static_features[-1].shape[0]
+
+    def _embedders(self):
+        return {"mesh": (self.mesh_embedders, self.mesh_static_features),
+                "mesh_up": (self.mesh_up_embedders, self.mesh_up_features),
+                "mesh_down": (self.mesh_down_embedders, self.mesh_down_features),
+                "m2m": (self.m2m_embedders if self.embedd_m2m else [], self.m2m_features)}
+
+    def _static_params(self):
+        mods = [self.g2m_embedder, self.m2g_embedder] + [m for embs, _ in self._embedders().values() for m in embs]
+        return [p for m in mods for p in m.parameters()]
+
+    def _compute_static(self):
+        st = {"g2m": self.g2m_embedder(self.g2m_features), "m2g": self.m2g_embedder(self.m2g_features)}
+        for k, (embs, feats) in self._embedders().items():
+            st[k] = [e(f) for e, f in zip(embs, feats)]
+        return st
+
+    def _graph_emb(self, batch_size):
+        ex = lambda t: self.expand_to_batch(t, batch_size)  # noqa: E731
+        return {k: ([ex(t) for t in v] if isinstance(v, list) else ex(v)) for k, v in self.static_embeddings().items()}
+
+    def embedd_mesh(self, batch_size):
+        """``mesh``, ``m2m`` (empty without intra-level layers), ``mesh_up`` and ``mesh_down`` embeddings per level, expanded
+        to the batch (graph_efm.py:746-793)."""
+        ge = self._graph_emb(batch_size)
+        return {k: ge[k] for k in ("mesh", "mesh_up", "mesh_down", "m2m")}
+
+    @torch.no_grad()
+    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
+        """The no-grad step: (1) grid embedder, decoder grid MLP and the projections of both g2m layers (the prior's and the
+        decoder's: both have the static level-0 embedding as receivers) in one launch, then both g2m layers on their
+        projections, (2) the prior's sweep up the hierarchy, (3) prior parameters + sample + latent embedding in one launch,
+        (4) the decoder's up and down sweeps, (5) m2g + param_map + step epilogue.  With a constant prior the launch of (1)
+        serves the decoder's g2m alone.  Each fused launch falls back to its composition where the library does not cover
+        the shapes."""
+        B = prev_state.shape[0]
+        ge = self._graph_emb(B)
+        prior, dec = self.prior_model, self.decoder
+        learned = isinstance(prior, HiGraphLatentEncoder)
+        sources = self._grid_sources(prev_state, prev_prev_state, forcing)
+        mesh0, g2m = ge["mesh"][0], ge["g2m"]
+        grid_emb = prior_rep = None
+        if learned:
+            enc = prior.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0, g2m,
+                                            second=dec.g2m_gnn)
+            if enc is not None:
+                prior_rep, res_grid, dec_rep = enc
+        else:
+            enc = dec.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0, g2m)
+            if enc is not None:
+                dec_rep, res_grid = enc
+        if enc is None:
+            grid_emb = self.grid_prev_embedder.apply_rows(sources)
+            res_grid = dec.grid_update_mlp.apply_rows([grid_emb], res=grid_emb)
+            prior_rep = prior.g2m_gnn(grid_emb, mesh0, g2m) if learned else None
+            dec_rep = dec.g2m_gnn(grid_emb, mesh0, g2m)
+        eps = self._noise(latent_noise, B, prev_state.device)
+        if learned:
+            prior_rep = prior.process_mesh(prior_rep, ge)
+        elif grid_emb is None:  # the constant prior reads only the batch size and device of its input
+            grid_emb = res_grid
+        latent_emb = self._sample_latent(prior_rep, grid_emb, eps)
+        mesh_rep = dec.mesh_step(dec_rep, latent_emb, ge)
+        return self._decode(mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
 
 
 MODELS = {"graph_lam": GraphLAM, "hi_lam": HiLAM, "hi_lam_parallel": HiLAMParallel}
@@ -793,7 +955,7 @@ class ARForecaster(nn.Module):
         if getattr(p, "samples_latent", False):
             # a predictor that samples: every captured step first refills this buffer from the default generator of the
             # device, so each replay draws fresh noise and torch.cuda.manual_seed makes a sequence of replays reproducible
-            bufs["latent_noise"] = torch.zeros(batch_size, p.num_mesh_nodes, p.latent_dim, device=dev)
+            bufs["latent_noise"] = torch.zeros(batch_size, p.latent_spatial_dim, p.latent_dim, device=dev)
         p.static_embeddings()  # materialise the weight-only embeddings outside the graph
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))

@@ -114,18 +114,23 @@ class GNNSequential(nn.Module):
     def __getitem__(self, i):
         return getattr(self, f"module_{i}")
 
-    def forward(self, mesh_rep, edge_rep, keep_edge_rep=True):
+    def forward(self, mesh_rep, edge_rep, keep_edge_rep=True, keep_stacked=False):
         """``keep_edge_rep=False``: the caller discards the final edge representation (GraphLAM.process_step,
         reference graph_lam.py:185 ``mesh_rep, _ = self.processor(...)``): in no-grad mode the last layer then
-        skips writing it, and the layers in between update their (private) edge tensor IN PLACE."""
-        fast = (not keep_edge_rep) and not torch.is_grad_enabled()
+        skips writing it, and the layers in between update their (private) edge tensor IN PLACE.
+        ``keep_stacked=True``: the same stacked path in no-grad mode, but the final edge representation is returned: the
+        last layer writes it in place into the stack's private tensor (out of place when it is also the first layer, whose
+        input belongs to the caller).  Graph-EFM's hierarchical decoder hands it to its down sweep."""
+        grad = torch.is_grad_enabled()
+        fast = (keep_stacked or not keep_edge_rep) and not grad
+        keep = keep_stacked or keep_edge_rep
         proj = None  # node projections of the next layer's edge MLP, computed by the previous layer's node kernel
         for i in range(self._n):
             mod = getattr(self, f"module_{i}")
             if fast and hasattr(mod, "forward_stacked"):
                 nxt = getattr(self, f"module_{i + 1}") if i + 1 < self._n else None
                 mesh_rep, edge_rep, proj = mod.forward_stacked(mesh_rep, edge_rep, first=(i == 0), last=(i == self._n - 1),
-                                                               proj_in=proj, next_layer=nxt)
+                                                               proj_in=proj, next_layer=nxt, keep_edges=keep)
             else:
                 assert proj is None
                 mesh_rep, edge_rep = mod(mesh_rep, mesh_rep, edge_rep)

@@ -518,17 +518,20 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
     return out
 
 
-def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=0, want_emb=False):
+def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=0, want_emb=False, edge_seq_b=None):
     """The grid side of a forecast step's encoder in ONE launch (``nlam_encode_fwd``): ``grid_emb = embed_seq(cat sources)``
     stays on chip; returns ``(grid_rep, proj)`` with ``grid_rep = grid_emb + grid_seq(grid_emb)`` (B, G, 64) and
     ``proj = [P_s | P_r]`` flat, ``P_s = grid_emb·W1sᵀ`` (B, G, 64) and ``P_r = mesh·W1rᵀ + b1`` (n_mesh, 64) of the grid -> mesh
     layer's edge MLP ``edge_seq`` on ``graph`` — the ``proj_in`` of that layer's ``inet_fwd`` with send = P_s.  ``mesh`` and
     ``edge_csr`` are shared by the batch.  ``want_emb``: also store grid_emb (``nlam_encode_emb_fwd``) and return
-    ``(grid_rep, proj, grid_emb)``.  Returns None when the library does not fuse these shapes / this math mode (the
-    caller then runs the embedder, the g2m layer and ``grid_seq`` as three calls)."""
+    ``(grid_rep, proj, grid_emb)``.  ``edge_seq_b``: the edge MLP of a second grid -> mesh layer on the same graph, receivers
+    and edge features (``nlam_encode2_fwd``); returns ``(grid_rep, proj, proj_b)`` with that layer's projections.  Returns
+    None when the library does not fuse these shapes / this math mode (the caller then runs the embedder, the g2m layer(s)
+    and ``grid_seq`` as separate calls)."""
     L = _lib.lib()
     if flags & _lib.MATH_FP32:
         return None
+    assert not (want_emb and edge_seq_b is not None), "encode: grid_emb is not stored with a second edge MLP"
     prepared = [as_rows(t) for t in sources]
     m, Bm, mbs = as_rows(mesh)
     e, Be, ebs = as_rows(edge_csr)
@@ -551,7 +554,12 @@ def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=
     args = (m.data_ptr(), mbs if Bm > 1 else 0, e.data_ptr(), ebs if Be > 1 else 0, grid_rep.data_ptr(), proj.data_ptr())
     grid_emb = torch.empty((B, G, 64), device=m.device, dtype=torch.float32) if want_emb else None
     with torch.cuda.device(m.device):
-        if want_emb:
+        if edge_seq_b is not None:
+            sm_b = mlp_struct(edge_seq_b)
+            proj_b = torch.empty_like(proj)
+            rc = L.nlam_encode2_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
+                                    ctypes.byref(sm_b), *args, proj_b.data_ptr(), G, B, flags, _stream_ptr(m.device))
+        elif want_emb:
             rc = L.nlam_encode_emb_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
                                        *args, grid_emb.data_ptr(), G, B, flags, _stream_ptr(m.device))
         else:
@@ -560,6 +568,8 @@ def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=
     if rc == _lib.E_UNSUPPORTED:
         return None
     _lib.check(rc)
+    if edge_seq_b is not None:
+        return grid_rep, proj, proj_b
     return (grid_rep, proj, grid_emb) if want_emb else (grid_rep, proj)
 
 
