@@ -250,6 +250,21 @@ int nlam_latent_sample_supported(const NlamMlp* param_mlp, const NlamMlp* embed_
                                  const float* eps, int64_t eps_bstride, const float* latent_emb, int64_t n_rows, int B, int flags);
 int nlam_latent_sample_fwd(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bstride, const float* eps,
                            int64_t eps_bstride, float* latent_emb, int64_t n_rows, int B, int flags, void* stream);
+/* Statistics of an ensemble of K forecast members (csrc/ensemble.cu, DESIGN §4.5).  members (B, K, G, d): member k of
+ * initial condition b starts at members + b*member_bstride + k*member_kstride (elements) and holds a dense (G, d) block, so
+ * rows b*K + k of a forecast batch and a time slice of a (B, K, T, G, d) tensor both qualify.  Per point, x_1..x_K its
+ * members and y = target[b*target_bstride + g*d + v]:
+ *   mean = (1/K) Σ x_k,   std = sqrt((1/(K-1)) Σ (x_k - mean)²)                     (B, G, d) dense
+ *   SE = (mean - y)²,  s² = std²,  A = (1/K) Σ |x_k - y|,  D = (1/(K(K-1))) Σ_{k≠l} |x_k - x_l|
+ * scores (B, d, 4) (NULL: not computed; then target, interior and the workspace may be NULL) holds the means of
+ * [SE, s², A, D] over the interior grid nodes (interior[g] != 0; the reference's interior_mask_bool).  Exact fp32; the grid
+ * reduction is two-stage in a fixed order (no atomics): bit-reproducible, and row b's results do not depend on the other
+ * rows.  2 <= K <= 64, else NLAM_E_UNSUPPORTED.  workspace: nlam_ensemble_stats_workspace_bytes(B, G, d) bytes when
+ * scores is given. */
+size_t nlam_ensemble_stats_workspace_bytes(int B, int64_t G, int d);
+int nlam_ensemble_stats(const float* members, int64_t member_bstride, int64_t member_kstride, int B, int K, int64_t G, int d,
+                        const float* target, int64_t target_bstride, const float* interior, float* mean, float* std,
+                        float* scores, void* workspace, size_t ws_bytes, void* stream);
 /* out[b,n,:] = scale_n * sum_{k in [ptr[n],ptr[n+1])} x[b, order ? order[k] : k, :]
  * scale_n = 1 (sum) or 1/max(deg,1) (mean).  Deterministic, CSR order. */
 int nlam_segment_sum(const int32_t* ptr, const int32_t* order, int64_t n_seg, const float* x,

@@ -363,3 +363,16 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
     return tc_rowmlp(aggr_mlp, nsrcs, 2, &nres, rec_out, g->n_rec, B, st);
   return rowmlp_simt(aggr_mlp, nsrcs, 2, &nres, nullptr, rec_out, nullptr, g->n_rec, B, st);
 }
+
+extern "C" size_t nlam_ensemble_stats_workspace_bytes(int B, int64_t G, int d) {
+  return (B >= 1 && G >= 1 && d >= 1) ? ens_stats_workspace_bytes(B, G, d) : 0;
+}
+
+extern "C" int nlam_ensemble_stats(const float* members, int64_t member_bstride, int64_t member_kstride, int B, int K,
+                                   int64_t G, int d, const float* target, int64_t target_bstride, const float* interior,
+                                   float* mean, float* std, float* scores, void* workspace, size_t ws_bytes, void* stream) {
+  NLAM_REQUIRE(members && mean && std && B >= 1 && G >= 1 && d >= 1, NLAM_E_INVALID, "nlam_ensemble_stats: bad arguments");
+  NLAM_REQUIRE(!scores || (target && interior), NLAM_E_INVALID, "nlam_ensemble_stats: scores need a target and an interior mask");
+  return ens_stats(members, member_bstride, member_kstride, B, K, G, d, target, target_bstride, interior, mean, std, scores,
+                   workspace, ws_bytes, (cudaStream_t)stream);
+}

@@ -203,6 +203,11 @@ inline double edge_algorithmic_bytes(const NlamGraph* g, int B, int64_t send_bs,
          4.0 * g->n_edges + 4.0 * (g->n_rec + 1) + 4.0 * (4.0 * H * H + 5.0 * H);
 }
 
+// ensemble.cu: ensemble mean / spread per point and interior-mean scores of K members (nlam_ensemble_stats)
+size_t ens_stats_workspace_bytes(int B, int64_t G, int d);
+int ens_stats(const float* x, int64_t x_bs, int64_t x_ks, int B, int K, int64_t G, int d, const float* y, int64_t y_bs,
+              const float* interior, float* mean, float* std, float* scores, void* ws, size_t ws_bytes, cudaStream_t st);
+
 // simt.cu
 int rowmlp_simt(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res,
                 const NlamRowSrc* res2, float* out, float* out2, int64_t n_rows, int B,

@@ -22,7 +22,7 @@ import ctypes
 import torch
 from torch import nn
 
-from . import _lib, ops
+from . import _lib, ensemble, ops
 from .gnn_layers import InteractionNet, get_gnn_class
 from . import clamping
 from .latent import (ConstantLatentEncoder, GraphLatentDecoder, GraphLatentEncoder, HiGraphLatentDecoder,
@@ -948,6 +948,21 @@ class ARForecaster(nn.Module):
         rotations are three graphs sharing one memory pool.  Returns the dict of static buffers
         (``forcing``, ``boundary``, ``state``)."""
         p = self.predictor
+        bufs = self._step_buffers(batch_size)
+        p.static_embeddings()  # materialise the weight-only embeddings outside the graph
+        graphs = self._capture_ring(lambda k: self._one_step(bufs, k))
+        self._graph = (batch_size, graphs, bufs)
+        # the graphs hold the cached static embeddings and every weight BY ADDRESS: remember what they were captured
+        # against so that a later weight update / load_state_dict / .to() triggers a re-capture instead of a stale replay
+        self._graph_key = self._capture_key(batch_size)
+        self._graph_static = p._static_cache  # keeps the captured embedding tensors alive while the graphs exist
+        self._phase = 0
+        return bufs
+
+    def _step_buffers(self, batch_size):
+        """The static buffers of a captured step on ``batch_size`` rows: ``forcing``, ``boundary``, the ``state`` ring and,
+        for a sampling predictor, ``latent_noise``."""
+        p = self.predictor
         dev = self.boundary_mask.device
         G, d, f = p.num_grid_nodes, p.num_state_vars, p.grid_input_dim - 2 * p.num_state_vars - p.grid_static_features.shape[1]
         bufs = {"forcing": torch.zeros(batch_size, G, f, device=dev), "boundary": torch.zeros(batch_size, G, d, device=dev),
@@ -956,27 +971,26 @@ class ARForecaster(nn.Module):
             # a predictor that samples: every captured step first refills this buffer from the default generator of the
             # device, so each replay draws fresh noise and torch.cuda.manual_seed makes a sequence of replays reproducible
             bufs["latent_noise"] = torch.zeros(batch_size, p.latent_spatial_dim, p.latent_dim, device=dev)
-        p.static_embeddings()  # materialise the weight-only embeddings outside the graph
+        return bufs
+
+    def _capture_ring(self, step):
+        """Warm ``step(0)`` up twice on a side stream, then capture ``step(k)`` for the three rotations of the state ring
+        into three CUDA graphs sharing one memory pool."""
+        dev = self.boundary_mask.device
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(2):  # warm up allocator / lazy handles
-                self._one_step(bufs, 0)
+                step(0)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         graphs = []
         for k in range(3):
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, pool=graphs[0].pool() if graphs else None):
-                self._one_step(bufs, k)
+                step(k)
             graphs.append(g)
-        self._graph = (batch_size, graphs, bufs)
-        # the graphs hold the cached static embeddings and every weight BY ADDRESS: remember what they were captured
-        # against so that a later weight update / load_state_dict / .to() triggers a re-capture instead of a stale replay
-        self._graph_key = self._capture_key(batch_size)
-        self._graph_static = p._static_cache  # keeps the captured embedding tensors alive while the graphs exist
-        self._phase = 0
-        return bufs
+        return graphs
 
     def _capture_key(self, batch_size):
         p = self.predictor
@@ -1027,6 +1041,89 @@ class ARForecaster(nn.Module):
             bufs["boundary"].copy_(boundary_states[:, i])
             out[:, i].copy_(self.replay_step())
         return out
+
+    # ---- ensemble forecasts of a sampling predictor: K members per initial condition, reduced on the device ----------
+    def _capture_ensemble(self, B, K, with_scores):
+        """Capture the ensemble step for B initial conditions of K members: expand the step's forcing and boundary
+        (B rows each) to the B·K member rows in one broadcast copy each, run the predictor step on the B·K rows with fresh
+        noise (``_one_step``, as ``capture`` does) and reduce the new states with ``ens_stats_kernel``.  Kept apart from
+        ``capture``'s graphs: neither evicts the other."""
+        p = self.predictor
+        dev = self.boundary_mask.device
+        bufs = self._step_buffers(B * K)
+        G, d, f = bufs["boundary"].shape[1], bufs["boundary"].shape[2], bufs["forcing"].shape[2]
+        bufs.update({"ens_forcing": torch.zeros(B, G, f, device=dev), "ens_boundary": torch.zeros(B, G, d, device=dev),
+                     "mean": torch.zeros(B, G, d, device=dev), "std": torch.zeros(B, G, d, device=dev)})
+        if with_scores:
+            bufs.update({"target": torch.zeros(B, G, d, device=dev), "scores": torch.zeros(B, d, 4, device=dev),
+                         "workspace": torch.zeros(ensemble.workspace_bytes(B, G, d), dtype=torch.uint8, device=dev)})
+        interior = self.interior_mask.reshape(-1).contiguous()
+
+        def step(k):
+            bufs["forcing"].view(B, K, G, f).copy_(bufs["ens_forcing"].unsqueeze(1).expand(B, K, G, f))
+            bufs["boundary"].view(B, K, G, d).copy_(bufs["ens_boundary"].unsqueeze(1).expand(B, K, G, d))
+            self._one_step(bufs, k)
+            ensemble.launch(bufs["state"][(k + 2) % 3].view(B, K, G, d), interior, bufs["mean"], bufs["std"],
+                            target=bufs.get("target"), scores=bufs.get("scores"), workspace=bufs.get("workspace"))
+
+        p.static_embeddings()
+        graphs = self._capture_ring(step)
+        self._ens = {"key": (B, K, with_scores) + self._capture_key(B * K), "graphs": graphs, "bufs": bufs,
+                     "static": p._static_cache, "interior": interior}
+
+    @torch.no_grad()
+    def rollout_ensemble(self, init_states, forcing_features, boundary_states, members, targets=None):
+        """Ensemble forecast of a sampling predictor (Graph-EFM), reduced on the device: ``members`` forecasts per initial
+        condition, each with its own latent noise, of which only the ensemble mean and spread are stored.
+
+        ``init_states`` (B, 2, G, d), ``forcing_features`` (B, T, G, f), ``boundary_states`` (B, T, G, d) and the optional
+        ``targets`` (B, T, G, d) are per initial condition, on the device.  Returns ``(mean, std, scores)``: mean and std
+        (B, T, G, d) over the members (``ensemble.ensemble_stats``), and with ``targets`` an ``ensemble.EnsembleScores`` of
+        (B, T, d) interior-grid means, else None.  In the reference's evaluation loop the targets are the boundary tensor
+        (module.py:389-391), so the same tensor may be passed twice.
+
+        Each step replays one captured graph: the member expansion of that step's forcing and boundary, the predictor step
+        on B·members rows with fresh noise per replay (as ``rollout_graphed`` draws it: after the same
+        ``torch.cuda.manual_seed`` the members are ``rollout_graphed``'s rows on the inputs expanded to B·members rows) and
+        ``ens_stats_kernel``.  Only B rows of forcing and boundary enter per step."""
+        p = self.predictor
+        if not getattr(p, "samples_latent", False):
+            raise ValueError(f"rollout_ensemble needs a predictor that samples its latent (Graph-EFM), got {type(p).__name__}")
+        if isinstance(members, bool) or not isinstance(members, int) or not 2 <= members <= ensemble.MAX_MEMBERS:
+            raise ValueError(f"rollout_ensemble: members must be an int in 2 .. {ensemble.MAX_MEMBERS}, got {members!r}")
+        G, d = p.num_grid_nodes, p.num_state_vars
+        if forcing_features.dim() != 4 or forcing_features.shape[2] != G:
+            raise ValueError(f"forcing_features: expected (B, T, {G}, f), got {tuple(forcing_features.shape)}")
+        B, T = forcing_features.shape[0], forcing_features.shape[1]
+        want = {"init_states": (init_states, (B, 2, G, d)), "boundary_states": (boundary_states, (B, T, G, d))}
+        if targets is not None:
+            want["targets"] = (targets, (B, T, G, d))
+        for name, (t, shape) in want.items():
+            if tuple(t.shape) != shape:
+                raise ValueError(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
+        K, with_scores = members, targets is not None
+        ens = getattr(self, "_ens", None)
+        if ens is None or ens["key"] != (B, K, with_scores) + self._capture_key(B * K):
+            self._capture_ensemble(B, K, with_scores)
+        graphs, bufs = self._ens["graphs"], self._ens["bufs"]
+        dev = init_states.device
+        mean = torch.empty(B, T, G, d, device=dev)
+        std = torch.empty(B, T, G, d, device=dev)
+        scores = torch.empty(B, T, d, 4, device=dev) if with_scores else None
+        st = bufs["state"]
+        st[0].view(B, K, G, d).copy_(init_states[:, 0].unsqueeze(1).expand(B, K, G, d))
+        st[1].view(B, K, G, d).copy_(init_states[:, 1].unsqueeze(1).expand(B, K, G, d))
+        for i in range(T):
+            bufs["ens_forcing"].copy_(forcing_features[:, i])
+            bufs["ens_boundary"].copy_(boundary_states[:, i])
+            if with_scores:
+                bufs["target"].copy_(targets[:, i])
+            graphs[i % 3].replay()
+            mean[:, i].copy_(bufs["mean"])
+            std[:, i].copy_(bufs["std"])
+            if with_scores:
+                scores[:, i].copy_(bufs["scores"])
+        return mean, std, (ensemble.EnsembleScores.from_means(scores, K) if with_scores else None)
 
     @torch.no_grad()
     def host_io_bytes_per_step(self, B):
