@@ -265,6 +265,18 @@ size_t nlam_ensemble_stats_workspace_bytes(int B, int64_t G, int d);
 int nlam_ensemble_stats(const float* members, int64_t member_bstride, int64_t member_kstride, int B, int K, int64_t G, int d,
                         const float* target, int64_t target_bstride, const float* interior, float* mean, float* std,
                         float* scores, void* workspace, size_t ws_bytes, void* stream);
+/* Gradient of nlam_ensemble_stats' interior means with respect to the members (csrc/ensemble.cu, DESIGN §4.5).  members,
+ * target and interior as in nlam_ensemble_stats.  grad_means (B, d, 4) contiguous: the upstream gradients of the means of
+ * [SE, s², A, D], already divided by N, the number of interior grid nodes (so the call needs no count on the host).
+ * grad_members (B, K, G, d) dense receives, at an interior point,
+ *   g_k = grad_SE · 2(mean - y)/K + grad_s² · 2(x_k - mean)/(K-1) + grad_A · sign(x_k - y)/K
+ *       + grad_D · 2/(K(K-1)) · Σ_{l≠k} sign(x_k - x_l)                                  with sign(0) = 0
+ * and 0 at a boundary node.  mean is formed as in the forward (identical members give an exact 0 in the s² and D terms).
+ * Every output is a function of its own point: bit-reproducible, and row b's gradient does not depend on the other rows.
+ * 2 <= K <= 64, else NLAM_E_UNSUPPORTED. */
+int nlam_ensemble_stats_bwd(const float* members, int64_t member_bstride, int64_t member_kstride, int B, int K, int64_t G, int d,
+                            const float* target, int64_t target_bstride, const float* interior, const float* grad_means,
+                            float* grad_members, void* stream);
 /* out[b,n,:] = scale_n * sum_{k in [ptr[n],ptr[n+1])} x[b, order ? order[k] : k, :]
  * scale_n = 1 (sum) or 1/max(deg,1) (mean).  Deterministic, CSR order. */
 int nlam_segment_sum(const int32_t* ptr, const int32_t* order, int64_t n_seg, const float* x,

@@ -376,3 +376,12 @@ extern "C" int nlam_ensemble_stats(const float* members, int64_t member_bstride,
   return ens_stats(members, member_bstride, member_kstride, B, K, G, d, target, target_bstride, interior, mean, std, scores,
                    workspace, ws_bytes, (cudaStream_t)stream);
 }
+
+extern "C" int nlam_ensemble_stats_bwd(const float* members, int64_t member_bstride, int64_t member_kstride, int B, int K,
+                                       int64_t G, int d, const float* target, int64_t target_bstride, const float* interior,
+                                       const float* grad_means, float* grad_members, void* stream) {
+  NLAM_REQUIRE(members && target && interior && grad_means && grad_members && B >= 1 && G >= 1 && d >= 1, NLAM_E_INVALID,
+               "nlam_ensemble_stats_bwd: bad arguments");
+  return ens_stats_bwd(members, member_bstride, member_kstride, B, K, G, d, target, target_bstride, interior, grad_means,
+                       grad_members, (cudaStream_t)stream);
+}

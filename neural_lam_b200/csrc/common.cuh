@@ -207,6 +207,8 @@ inline double edge_algorithmic_bytes(const NlamGraph* g, int B, int64_t send_bs,
 size_t ens_stats_workspace_bytes(int B, int64_t G, int d);
 int ens_stats(const float* x, int64_t x_bs, int64_t x_ks, int B, int K, int64_t G, int d, const float* y, int64_t y_bs,
               const float* interior, float* mean, float* std, float* scores, void* ws, size_t ws_bytes, cudaStream_t st);
+int ens_stats_bwd(const float* x, int64_t x_bs, int64_t x_ks, int B, int K, int64_t G, int d, const float* y, int64_t y_bs,
+                  const float* interior, const float* gup, float* grad, cudaStream_t st);
 
 // simt.cu
 int rowmlp_simt(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res,

@@ -131,6 +131,70 @@ __global__ void __launch_bounds__(kEnsThreads) ens_reduce_kernel(const float* __
   if (threadIdx.x == 0) out[((long long)b * d + var_i) * 4 + q] = sv[0] / (float)sc[0];
 }
 
+// Gradient of the four interior means with respect to the members (DESIGN §4.5).  gup (B, d, 4) holds the upstream
+// gradients of [SE, s², A, D] already divided by the interior count N, so at an interior point
+//   dL/dx_k = gup_SE · 2(m - y)/K + gup_var · 2(x_k - m)/(K-1) + gup_A · sign(x_k - y)/K
+//           + gup_D · 2/(K(K-1)) · Σ_{l≠k} sign(x_k - x_l)
+// and 0 at a boundary node (sign(0) = 0, torch's abs backward).  One point per thread, the K values in registers as in the
+// forward (m shifted by the first member: identical members give x_k - m = 0 exactly); the pair sign sum is an exact
+// integer count.  Every output depends on its own point only: no atomics, no reduction across points.  The gradient is
+// written dense, (B, K, G, d).
+template <int KMAX>
+__global__ void __launch_bounds__(kEnsThreads) ens_stats_bwd_kernel(const float* __restrict__ x, long long x_bs, long long x_ks,
+                                                                    int K, const float* __restrict__ y, long long y_bs,
+                                                                    const float* __restrict__ interior, long long n_pts, int d,
+                                                                    const float* __restrict__ gup, float* __restrict__ grad) {
+  const int b = blockIdx.y;
+  const long long p = (long long)blockIdx.x * kEnsThreads + threadIdx.x;
+  if (p >= n_pts) return;
+  float* gp = grad + (long long)b * K * n_pts + p;
+  if (interior[p / d] == 0.f) {
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+      if (k >= K) break;
+      gp[k * n_pts] = 0.f;
+    }
+    return;
+  }
+  float v[KMAX];
+  const float* xp = x + b * x_bs + p;
+#pragma unroll
+  for (int k = 0; k < KMAX; ++k) {
+    if (k >= K) break;
+    v[k] = __ldg(xp + k * x_ks);
+  }
+  const float c = v[0];
+  float su = 0.f;
+#pragma unroll
+  for (int k = 0; k < KMAX; ++k) {
+    if (k >= K) break;
+    su += v[k] - c;
+  }
+  const float mu = su / (float)K;
+  const float m = c + mu;
+  const float t = y[b * y_bs + p];
+  const float* g4 = gup + ((long long)b * d + (int)(p % d)) * 4;
+  const float fk = (float)K;
+  const float c_se = g4[0] * 2.f * (m - t) / fk;
+  const float c_var = g4[1] * 2.f / (fk - 1.f);
+  const float c_a = g4[2] / fk;
+  const float c_d = g4[3] * 2.f / (fk * (fk - 1.f));
+#pragma unroll
+  for (int k = 0; k < KMAX; ++k) {
+    if (k >= K) break;
+    const float vk = v[k];
+    int cnt = 0;  // Σ_{l≠k} sign(x_k - x_l); l = k adds 0
+#pragma unroll
+    for (int l = 0; l < KMAX; ++l) {
+      if (l >= K) break;
+      cnt += (int)(v[l] < vk) - (int)(v[l] > vk);
+    }
+    const float sa = (float)((int)(vk > t) - (int)(vk < t));
+    const float e = (vk - c) - mu;
+    gp[k * n_pts] = ((c_se + c_var * e) + c_a * sa) + c_d * (float)cnt;
+  }
+}
+
 static long long ens_ctas(long long n_pts) { return (n_pts + kEnsThreads - 1) / kEnsThreads; }
 
 size_t ens_stats_workspace_bytes(int B, int64_t G, int d) {
@@ -173,6 +237,30 @@ int ens_stats(const float* x, int64_t x_bs, int64_t x_ks, int B, int K, int64_t 
     count_launch();
     NLAM_CUDA_OK(cudaGetLastError());
   }
+  return NLAM_OK;
+}
+
+int ens_stats_bwd(const float* x, int64_t x_bs, int64_t x_ks, int B, int K, int64_t G, int d, const float* y, int64_t y_bs,
+                  const float* interior, const float* gup, float* grad, cudaStream_t st) {
+  NLAM_REQUIRE(K >= 2 && K <= 64, NLAM_E_UNSUPPORTED, "nlam_ensemble_stats_bwd: K = %d members outside 2 .. 64", K);
+  const long long n_pts = (long long)G * d, n_cta = ens_ctas(n_pts);
+  NLAM_REQUIRE(n_cta <= 0x7fffffff && B <= 65535, NLAM_E_UNSUPPORTED,
+               "nlam_ensemble_stats_bwd: G = %lld, d = %d, B = %d too large", (long long)G, d, B);
+  const dim3 grid((unsigned)n_cta, (unsigned)B);
+  {
+    // algorithmic bytes: the K members and the target read once, the K gradients written once
+    ProfScope ps("ens_stats_bwd_kernel", st, 4.0 * B * n_pts * (2 * K + 1));
+#define NLAM_ENS_BWD_LAUNCH(KM) \
+  ens_stats_bwd_kernel<KM><<<grid, kEnsThreads, 0, st>>>(x, x_bs, x_ks, K, y, y_bs, interior, n_pts, d, gup, grad)
+    if (K <= 4) NLAM_ENS_BWD_LAUNCH(4);
+    else if (K <= 8) NLAM_ENS_BWD_LAUNCH(8);
+    else if (K <= 16) NLAM_ENS_BWD_LAUNCH(16);
+    else if (K <= 32) NLAM_ENS_BWD_LAUNCH(32);
+    else NLAM_ENS_BWD_LAUNCH(64);
+#undef NLAM_ENS_BWD_LAUNCH
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
   return NLAM_OK;
 }
 

@@ -16,11 +16,15 @@ means are ``EnsembleScores``' properties: rmse = sqrt(mean SE), spread = sqrt(me
 ssr = sqrt((K+1)/K) · spread / rmse, the fair CRPS A - D/2 and the CRPS of the members' empirical distribution
 A - (K-1)/(2K) · D (both linear in A and D, so they can be formed after the grid average).
 
+``ensemble_stats`` is differentiable in the members through those four means (``ens_stats_bwd_kernel``), so the fair CRPS
+can serve as a training loss (``models.ARForecaster.efm_loss``).
+
 There is no CPU or eager fallback: CPU tensors, tensors that are not float32 and K outside 2 .. 64 raise.
 """
 from dataclasses import dataclass
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from .ops import _require_cuda, _stream_ptr
@@ -116,6 +120,57 @@ def launch(members, interior, mean, std, target=None, scores=None, workspace=Non
             std.data_ptr(), sp, wp, ws_bytes, _stream_ptr(members.device)))
 
 
+def launch_backward(members, interior, target, grad_means, grad_members):
+    """Gradient of ``launch``'s interior means with respect to the members (``ens_stats_bwd_kernel``).  ``members``,
+    ``interior`` and ``target`` as in ``launch``; ``grad_means`` (B, d, 4) contiguous: the upstream gradients of the means of
+    [SE, s², A, D] divided by the number of interior nodes; ``grad_members`` (B, K, G, d) contiguous receives the gradient."""
+    B, K, G, d = members.shape
+    _check_members(K)
+    _require_cuda(members, interior, target, grad_means, grad_members)
+    if tuple(grad_means.shape) != (B, d, 4) or not grad_means.is_contiguous():
+        raise ValueError(f"grad_means: expected a contiguous ({B}, {d}, 4) tensor, got {tuple(grad_means.shape)}")
+    if tuple(grad_members.shape) != (B, K, G, d) or not grad_members.is_contiguous():
+        raise ValueError(f"grad_members: expected a contiguous {(B, K, G, d)} tensor, got {tuple(grad_members.shape)}")
+    with torch.cuda.device(members.device):
+        _lib.check(_lib.lib().nlam_ensemble_stats_bwd(
+            members.data_ptr(), members.stride(0), members.stride(1), B, K, G, d, target.data_ptr(), target.stride(0),
+            interior.data_ptr(), grad_means.data_ptr(), grad_members.data_ptr(), _stream_ptr(members.device)))
+
+
+def _stats(members, interior, target):
+    B, K, G, d = members.shape
+    mean = torch.empty(B, G, d, device=members.device)
+    std = torch.empty_like(mean)
+    scores = ws = None
+    if target is not None:
+        scores = torch.empty(B, d, 4, device=members.device)
+        ws = torch.empty(workspace_bytes(B, G, d), dtype=torch.uint8, device=members.device)
+    launch(members, interior, mean, std, target=target, scores=scores, workspace=ws)
+    return mean, std, scores
+
+
+class _StatsFunction(torch.autograd.Function):
+    """``launch`` with a target as an autograd node: differentiable in the members through the four interior means; mean and
+    std are non-differentiable outputs, the target and the mask get no gradient.  No double backward."""
+
+    @staticmethod
+    def forward(ctx, members, interior, target):
+        mean, std, scores = _stats(members, interior, target)
+        ctx.mark_non_differentiable(mean, std)
+        ctx.save_for_backward(members, interior, target)
+        return mean, std, scores
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, _grad_mean, _grad_std, grad_scores):
+        members, interior, target = ctx.saved_tensors
+        # the 1/N of the interior means, applied on the device: no host synchronisation
+        n = (interior != 0).sum().to(grad_scores.dtype)
+        grad = torch.empty(members.shape, device=members.device)
+        launch_backward(members, interior, target, (grad_scores / n).contiguous(), grad)
+        return grad, None, None
+
+
 def ensemble_stats(members, interior_mask, target=None):
     """Ensemble mean, spread and (with ``target``) scores of stored members.
 
@@ -123,7 +178,12 @@ def ensemble_stats(members, interior_mask, target=None):
     (B, K, G, d), or a time slice ``x[:, :, t]`` of a (B, K, T, G, d) ensemble, are read without a copy).
     ``interior_mask`` (G) or (G, 1): nonzero / True on the interior grid nodes the scores average over (the forecaster's
     ``interior_mask``).  ``target`` (B, G, d).  Returns ``(mean, std, scores)``: mean m and std s = sqrt(s²) as (B, G, d)
-    and an ``EnsembleScores`` of (B, d) tensors, or None without a target."""
+    and an ``EnsembleScores`` of (B, d) tensors, or None without a target.
+
+    With a target, grad mode on and ``members`` requiring grad, the scores are differentiable in ``members``
+    (``ens_stats_bwd_kernel``, DESIGN §4.5), so a loss built from them (e.g. ``crps_fair``) can be backpropagated; mean and
+    std are then returned as non-differentiable tensors, and ``target`` and the mask get no gradient.  Double backward is
+    not supported.  Otherwise the call is the plain forward launch."""
     members = _member_blocks(members)
     B, K, G, d = members.shape
     _check_members(K)
@@ -132,15 +192,13 @@ def ensemble_stats(members, interior_mask, target=None):
         interior = interior.float()
     _require_cuda(members, interior, target)
     interior = interior.contiguous()
-    mean = torch.empty(B, G, d, device=members.device)
-    std = torch.empty_like(mean)
-    scores = ws = None
     if target is not None:
         if target.dim() != 3:
             raise ValueError(f"target: expected (B, G, d), got shape {tuple(target.shape)}")
         if (d > 1 and target.stride(2) != 1) or (G > 1 and target.stride(1) != d):
             target = target.contiguous()
-        scores = torch.empty(B, d, 4, device=members.device)
-        ws = torch.empty(workspace_bytes(B, G, d), dtype=torch.uint8, device=members.device)
-    launch(members, interior, mean, std, target=target, scores=scores, workspace=ws)
+    if target is not None and torch.is_grad_enabled() and members.requires_grad:
+        mean, std, scores = _StatsFunction.apply(members, interior, target.detach())
+    else:
+        mean, std, scores = _stats(members, interior, target)
     return mean, std, (EnsembleScores.from_means(scores, K) if scores is not None else None)

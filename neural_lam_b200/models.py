@@ -18,6 +18,9 @@ is kept receiver-sorted, and input-independent embeddings are cached between ste
 weights do not change (SURVEY.md section 8f item 1).
 """
 import ctypes
+import math
+from dataclasses import dataclass
+from typing import Optional
 
 import torch
 from torch import nn
@@ -606,6 +609,27 @@ class BaseGraphEFM(BaseGraphModel):
         rescaled = mean_delta * self.diff_std + self.diff_mean
         return self.get_clamped_new_state(rescaled, prev_state), pred_std
 
+    def forward_posterior(self, prev_state, prev_prev_state, forcing, target_state, latent_noise=None):
+        """One step sampled from the variational posterior q(z | X_{t-1}, X_t, forcing, X_{t+1}) -> ``(new_state,
+        pred_std|None, kl)``.
+
+        q is ``self.encoder`` on ``embedd_grid_with_target`` (diagonal Gaussian), p is ``self.prior_model`` (learned
+        isotropic / diagonal or constant); z = mean_q + ε · std_q with ε = ``latent_noise`` (B, latent_spatial_dim,
+        latent_dim) or a ``torch.randn`` draw as in ``forward``; decoder and clamped update as in ``forward``.  ``kl`` (B,) is
+        the closed form KL(q ‖ p) = log(σ_p/σ_q) + (σ_q² + (μ_q - μ_p)²)/(2σ_p²) - ½, summed over the latent dimension and
+        averaged over the latent nodes (``latent_spatial_dim`` of them).  Composed from the autograd-capable modules, so it
+        trains every parameter it reads; it runs under ``no_grad`` as well."""
+        grid_emb, graph_emb = self.embedd_grid_and_graph(prev_state, prev_prev_state, forcing)
+        grid_cur = self.embedd_grid_with_target(prev_state, prev_prev_state, forcing, target_state)
+        q = self.encoder(grid_cur, graph_emb=graph_emb)
+        p = self.prior_model(grid_emb, graph_emb=graph_emb)
+        eps = self._noise(latent_noise, prev_state.shape[0], prev_state.device)
+        latent_samples = q.mean + eps * q.stddev
+        mean_delta, pred_std = self.decoder(grid_emb, latent_samples, graph_emb)
+        rescaled = mean_delta * self.diff_std + self.diff_mean
+        kl = (torch.log(p.stddev / q.stddev) + (q.variance + (q.mean - p.mean) ** 2) / (2 * p.variance) - 0.5)
+        return self.get_clamped_new_state(rescaled, prev_state), pred_std, kl.sum(dim=-1).mean(dim=-1)
+
     @torch.no_grad()
     def forward_with_boundary(self, prev_state, prev_prev_state, forcing, boundary_state, boundary_mask, latent_noise=None,
                               out=None):
@@ -909,6 +933,34 @@ def _boundary_blocks(mask, max_blocks=8, min_saving=0.2):
     return blocks
 
 
+@dataclass(frozen=True)
+class EFMLoss:
+    """Graph-EFM's training objective over an autoregressive rollout of T steps (``ARForecaster.efm_loss``): ``loss`` the
+    0-dim value to backpropagate, ``recon`` and ``kl`` (T,) per step, ``crps`` (T,) per step or None without the ensemble
+    term.  Every term is a mean over the batch."""
+    loss: torch.Tensor
+    recon: torch.Tensor
+    kl: torch.Tensor
+    crps: Optional[torch.Tensor]
+
+
+def _interior_mean(entry, interior):
+    """(B, G, d) per-entry values -> (B,): mean over the interior grid nodes, summed over the variables (the reference's
+    ``mask_and_reduce_metric(..., average_grid=True, sum_vars=True)``, metrics.py:37-84, with the mask as weights)"""
+    return (entry * interior).sum(dim=1).sum(dim=-1) / interior.sum()
+
+
+def _wmse(pred, target, std, interior):
+    """metrics.py ``wmse``: (pred - target)² / std², interior mean, summed over the variables -> (B,)"""
+    return _interior_mean((pred - target) ** 2 / std ** 2, interior)
+
+
+def _nll(pred, target, std, interior):
+    """metrics.py ``nll``: -log N(target; pred, std), interior mean, summed over the variables -> (B,)"""
+    entry = torch.log(std) + 0.5 * math.log(2 * math.pi) + (target - pred) ** 2 / (2 * std ** 2)
+    return _interior_mean(entry, interior)
+
+
 class ARForecaster(nn.Module):
     """Autoregressive rollout with boundary overwrite (reference
     models/forecasters/autoregressive.py:63-149).  ``forward`` keeps the reference semantics;
@@ -1124,6 +1176,86 @@ class ARForecaster(nn.Module):
             if with_scores:
                 scores[:, i].copy_(bufs["scores"])
         return mean, std, (ensemble.EnsembleScores.from_means(scores, K) if with_scores else None)
+
+    # ---- training objective of a sampling predictor (Graph-EFM) -------------------------------------------------------
+    def efm_loss(self, init_states, forcing_features, boundary_states, target_states, per_var_std, members=2, kl_weight=1.0,
+                 crps_weight=0.0, latent_noise=None):
+        """Graph-EFM's training objective (Oskarsson et al. 2024) over an autoregressive rollout of T steps -> ``EFMLoss``.
+
+        ``init_states`` (B, 2, G, d), ``forcing_features`` (B, T, G, f), ``boundary_states`` and ``target_states``
+        (B, T, G, d); ``per_var_std`` (d,) positive, the per-variable weights of the reference's loss (module.py:157-178).
+        Per step t, each term a mean over the batch:
+
+        * posterior branch (B rows): ``forward_posterior`` given ``target_states[:, t]``; its new state is boundary-mixed as
+          in ``forward`` and fed back.  ``recon[t]`` is the reference's ``wmse(pred, target, per_var_std, mask=interior)``,
+          or ``nll(pred, target, pred_std, mask)`` when the predictor outputs its std (module.py:492-504); ``kl[t]`` is the
+          posterior step's KL(q ‖ p);
+        * prior ensemble branch, only with ``crps_weight > 0`` (B·members rows, row b·members + k is member k of initial
+          condition b as in ``rollout_ensemble``): ``forward`` on the expanded inputs, each member fed back its own
+          boundary-mixed state.  ``crps[t]`` is the mean over b of Σ_v crps_fair[b, v] / per_var_std[v], the fair CRPS of
+          ``ensemble.ensemble_stats`` over the interior nodes (weighted as ``wmae`` weights the MAE).
+
+        ``loss`` = mean over t of recon[t] + kl_weight · kl[t] + crps_weight · crps[t].  ``latent_noise`` pins the draws:
+        ``(post_eps (T, B, N_lat, L), prior_eps (T, B·members, N_lat, L) or None)``; without it each step draws the
+        posterior's ε, then the members' ε, from the default generator of the device."""
+        p = self.predictor
+        if not getattr(p, "samples_latent", False):
+            raise ValueError(f"efm_loss needs a predictor that samples its latent (Graph-EFM), got {type(p).__name__}")
+        with_crps = crps_weight > 0
+        if with_crps and (isinstance(members, bool) or not isinstance(members, int)
+                          or not 2 <= members <= ensemble.MAX_MEMBERS):
+            raise ValueError(f"efm_loss: members must be an int in 2 .. {ensemble.MAX_MEMBERS}, got {members!r}")
+        G, d = p.num_grid_nodes, p.num_state_vars
+        if forcing_features.dim() != 4 or forcing_features.shape[2] != G:
+            raise ValueError(f"forcing_features: expected (B, T, {G}, f), got {tuple(forcing_features.shape)}")
+        B, T = forcing_features.shape[0], forcing_features.shape[1]
+        K = members
+        want = {"init_states": (init_states, (B, 2, G, d)), "boundary_states": (boundary_states, (B, T, G, d)),
+                "target_states": (target_states, (B, T, G, d))}
+        post_eps = prior_eps = None
+        if latent_noise is not None:
+            post_eps, prior_eps = latent_noise
+            lat = (p.latent_spatial_dim, p.latent_dim)
+            want["latent_noise[0]"] = (post_eps, (T, B) + lat)
+            if with_crps and prior_eps is not None:
+                want["latent_noise[1]"] = (prior_eps, (T, B * K) + lat)
+        for name, (t, shape) in want.items():
+            if tuple(t.shape) != shape:
+                raise ValueError(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
+        if tuple(per_var_std.shape) != (d,) or not bool((per_var_std > 0).all()):
+            raise ValueError(f"per_var_std: expected ({d},) positive values, got shape {tuple(per_var_std.shape)}")
+
+        interior = self.interior_mask.reshape(G, 1)
+        ex = lambda x: x.unsqueeze(1).expand(B, K, *x.shape[1:]).reshape(B * K, *x.shape[1:])  # noqa: E731
+        prev_prev, prev = init_states[:, 0], init_states[:, 1]
+        if with_crps:
+            ens_prev_prev, ens_prev = ex(init_states[:, 0]), ex(init_states[:, 1])
+            ens_forcing, ens_boundary = ex(forcing_features), ex(boundary_states)
+        recon, kl, crps = [], [], []
+        for t in range(T):
+            target = target_states[:, t]
+            pred, pred_std, step_kl = p.forward_posterior(prev, prev_prev, forcing_features[:, t], target,
+                                                          latent_noise=None if post_eps is None else post_eps[t])
+            new_state = self.boundary_mask * boundary_states[:, t] + self.interior_mask * pred
+            if pred_std is None:
+                recon.append(_wmse(new_state, target, per_var_std, interior).mean())
+            else:
+                recon.append(_nll(new_state, target, pred_std, interior).mean())
+            kl.append(step_kl.mean())
+            prev_prev, prev = prev, new_state
+            if with_crps:
+                ens_pred, _ = p(ens_prev, ens_prev_prev, ens_forcing[:, t],
+                                latent_noise=None if prior_eps is None else prior_eps[t])
+                ens_state = self.boundary_mask * ens_boundary[:, t] + self.interior_mask * ens_pred
+                _, _, scores = ensemble.ensemble_stats(ens_state.view(B, K, G, d), self.interior_mask, target)
+                crps.append((scores.crps_fair / per_var_std).sum(dim=-1).mean())
+                ens_prev_prev, ens_prev = ens_prev, ens_state
+        recon, kl = torch.stack(recon), torch.stack(kl)
+        total = recon + kl_weight * kl
+        crps = torch.stack(crps) if with_crps else None
+        if with_crps:
+            total = total + crps_weight * crps
+        return EFMLoss(loss=total.mean(), recon=recon, kl=kl, crps=crps)
 
     @torch.no_grad()
     def host_io_bytes_per_step(self, B):
