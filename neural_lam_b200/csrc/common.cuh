@@ -189,6 +189,7 @@ struct NlamGraph {
   // [rowptr[tile_rec[t]], rowptr[tile_rec[t+1]]).  n_tiles == 0 if some in-degree > 128.
   int32_t n_tiles = 0;
   int32_t* tile_rec = nullptr;  // n_tiles+1
+  int32_t* tile_edge = nullptr; // n_tiles+1: rowptr[tile_rec[t]], the first CSR edge of tile t
   int32_t ell_window = 0;       // 1: uniform in-degree <= 8 (the uniform-degree edge path)
   std::vector<int32_t> h_tile_rec, h_rowptr;
 };

@@ -2,7 +2,7 @@
 // edges of whole receivers), two warp groups own 64 rows each.  Per tile:
 //
 //   A  = [src_0 | src_1 | ...] rows (gathered through row indices, zero-padded to a multiple of 32 columns) -> shared memory
-//   h  = SiLU(A · W1ᵀ + b1 [+ P_s[src] + P_r[dst]])        wgmma, accumulators in registers, h back to shared memory
+//   h  = SiLU(A · W1ᵀ + b1)                                wgmma, accumulators in registers, h back to shared memory
 //   y  = LN(h · W2ᵀ + b2) [+ residual]                     wgmma
 //
 // then one of: the row output (optionally the forecast-step epilogue), the edge output e' = e + y together with the
@@ -13,11 +13,12 @@
 //
 // Launch names (nlam_profile_*): tc_rowmlp_kernel (row MLPs, node updates, output_map + step epilogue),
 // tc_rowlinear_kernel (node projections P_s = x_s·W1sᵀ, P_r = x_r·W1rᵀ + b1 of the split first edge Linear, both node
-// sets in one grid), tc_edge_kernel (K = 192 edge MLP on raw gathered rows), tc_edge3_kernel (split form, out-of-place
-// edge output), tc_edge_rmw_kernel (split form, edge tensor updated in place or not written), tc_ell_window_kernel
-// (uniform in-degree edge sets), tc_edge_bcast_kernel (batch-broadcast edge features and receivers, split form),
-// tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
-// epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).
+// sets in one grid), tc_edge_kernel (K = 192 edge MLP on raw gathered rows), tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
+// epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).  The split-form edge stage
+// (first edge Linear split into e·W1eᵀ and node projections gathered in its epilogue) runs in tc_edge_split_kernel below,
+// under the labels tc_edge3_kernel (out-of-place edge output), tc_edge_rmw_kernel (edge tensor updated in place or not
+// written), tc_ell_window_kernel (uniform in-degree edge sets) and tc_edge_bcast_kernel (batch-broadcast edge features
+// and receivers).
 #include "tc_ptx.cuh"
 #include "wgmma_tf32.cuh"
 
@@ -67,9 +68,6 @@ struct FzParams {
   const float *b1, *b2, *gamma, *beta, *b3, *b4;
   float eps;
   int act1, has_gemm2;
-  const float* add[2];  // gathered GEMM1 addends (rows of 64): add[a][b * add_bs[a] + add_idx[a][r] * 64 + c]
-  const int32_t* add_idx[2];
-  long long add_bs[2];
   const float* res;     // residual rows (64 wide)
   long long res_bs;
   float* out;           // (B, n_rows, out_w)
@@ -339,12 +337,6 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
       fz_store_rows(p, prob ? p.out_1 : p.out, 64, prob ? p.n_rows1 : p.n_rows, false, v, b, r0, valid0, valid1);
       continue;
     }
-    for (int a = 0; a < 2; ++a) {
-      if (!p.add[a]) continue;
-      const float* base = p.add[a] + (long long)b * p.add_bs[a];
-      fz_add_rows(v, valid0 ? base + (long long)__ldg(p.add_idx[a] + r0) * 64 : nullptr,
-                  valid1 ? base + (long long)__ldg(p.add_idx[a] + r0 + 8) * 64 : nullptr);
-    }
     if (p.act1) {
 #pragma unroll
       for (int i = 0; i < 2; ++i)
@@ -428,6 +420,232 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
     fz_unpack(acc, v, prm + 320);
     fz_store_rows(p, p.out, p.out_w, p.n_rows, true, v, b, r0, valid0, valid1);
   }
+}
+
+// ------------------------------------------------------------------------------------ split-form edge kernel
+// The edge stage of an InteractionNet layer whose first edge Linear is split, P_s = x_s·W1sᵀ and P_r = x_r·W1rᵀ + b1 given.
+// Per CSR tile (whole receivers, <= 128 edges) of batch element b, the arithmetic of fused_mlp_kernel's EDGE mode:
+//   m     = LN(SiLU(e·W1eᵀ + P_s[b, src[k]] + P_r[b, dst[k]])·W2ᵀ + b2)
+//   e'    = e + m                         (optional: out of place, in place, or not written)
+//   aggr  = sum (or mean) of m over each receiver's edges, k0 to k1 in CSR order
+// __launch_bounds__(256, 1): one persistent CTA per SM, each warp group owns 64 rows of the tile.  The whole load chain of
+// the next tile runs while this tile computes: its edge rows (one contiguous 16-byte aligned span per batch element) and
+// its rowptr entries are copied with cp.async into raw staging buffers before this tile's GEMMs, and its gathered P_s / P_r
+// rows right after this tile's GEMM 1 epilogue has read its own.  The tile bounds come two tiles ahead and the src / dst
+// indices one tile ahead, so no copy waits on the load of its address.  The raw staged e rows are rounded to TF32 (to
+// nearest) as they become the operand, and the residual e + m reads them from staging; the staging buffer then holds the
+// tile's messages for the per-receiver sums.
+namespace edg {
+using fz::CH_A;
+using fz::CH_W;
+constexpr int PITCH = 72;  // staged rows: 64 floats + 8 (fragment-layout float2 reads of a half warp hit distinct banks)
+constexpr uint32_t STG_BYTES = 128 * PITCH * 4;
+constexpr uint32_t W1 = 0, W2 = W1 + 2 * CH_W;
+constexpr uint32_t A = W2 + 2 * CH_W;          // 128 x 64 operand
+constexpr uint32_t STG = A + 2 * CH_A;         // two raw edge-row staging buffers (tiles of even / odd iteration)
+constexpr uint32_t PS = STG + 2 * STG_BYTES;   // staged P_s[src] rows of one tile
+constexpr uint32_t PR = PS + STG_BYTES;        // staged P_r[dst] rows of one tile
+constexpr uint32_t RP = PR + STG_BYTES;        // two copies of a tile's rowptr entries (<= 129)
+constexpr uint32_t PRM = RP + 2 * 132 * 4;     // b2 | gamma | beta
+constexpr uint32_t BYTES = PRM + 3 * 64 * 4 + 1024;  // + alignment slack
+static_assert(BYTES <= 227 * 1024, "edge kernel shared memory exceeds the sm_90 limit");
+}  // namespace edg
+
+struct EdgeParams {
+  int B, n_tiles, mean;
+  const int32_t *tile_rec, *tile_edge, *rowptr, *src, *dst;
+  const float* edge;     // (B | 1, n_edges, 64), batch stride edge_bs (0: shared by the batch)
+  long long edge_bs;
+  float* edge_out;       // NULL, edge (in place) or (B, n_edges, 64) dense
+  float* aggr;           // (B, n_rec, 64) dense
+  const float *ps, *pr;  // P_s (B | 1, n_send, 64), P_r (B | 1, n_rec, 64)
+  long long ps_bs, pr_bs;
+  FzW w1, w2;
+  const float *b2, *gamma, *beta;
+  float eps;
+  long long n_rec, n_edges;
+};
+
+struct EdgeTile {
+  int b, ra, rb, row0, nrows;  // b < 0: no such tile
+};
+
+__device__ __forceinline__ EdgeTile edge_tile(const EdgeParams& p, long long w, long long n_work) {
+  EdgeTile T{-1, 0, 0, 0, 0};
+  if (w < n_work) {
+    T.b = (int)(w / p.n_tiles);
+    const int t = (int)(w - (long long)T.b * p.n_tiles);
+    T.ra = __ldg(p.tile_rec + t);
+    T.rb = __ldg(p.tile_rec + t + 1);
+    T.row0 = __ldg(p.tile_edge + t);
+    T.nrows = __ldg(p.tile_edge + t + 1) - T.row0;
+  }
+  return T;
+}
+
+__global__ void __launch_bounds__(fz::THREADS, 1) tc_edge_split_kernel(const __grid_constant__ EdgeParams p) {
+  using namespace fz;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const uint32_t sb = smem_u32(s);
+  uint8_t* sA = s + edg::A;
+  float* prm = reinterpret_cast<float*>(s + edg::PRM);
+  const float* sps = reinterpret_cast<const float*>(s + edg::PS);
+  const float* spr = reinterpret_cast<const float*>(s + edg::PR);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
+  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // local row of fragment half 0 (half 1: + 8)
+  const int cq = 2 * (lane & 3);
+  const uint32_t aA = sb + edg::A + wg * (CH_A / 2);
+
+  fz_load_w(s + edg::W1, p.w1, 2, tid);
+  fz_load_w(s + edg::W2, p.w2, 2, tid);
+  for (int i = tid; i < 64; i += THREADS) {
+    prm[i] = p.b2 ? p.b2[i] : 0.f;
+    prm[64 + i] = p.gamma ? p.gamma[i] : 1.f;
+    prm[128 + i] = p.beta ? p.beta[i] : 0.f;
+  }
+
+  const long long n_work = (long long)p.n_tiles * p.B, stride = gridDim.x;
+  const uint64_t pol_stream = policy_evict_first(), pol_shared = policy_evict_normal();
+  const uint64_t pol_e = p.edge_bs ? pol_stream : pol_shared;
+  // the edge rows and rowptr entries of tile T -> staging buffer `buf`
+  auto issue_edges = [&](const EdgeTile& T, int buf) {
+    if (T.b < 0) return;
+    const float* g = p.edge + (long long)T.b * p.edge_bs + (long long)T.row0 * 64;
+    const uint32_t dst = sb + edg::STG + buf * edg::STG_BYTES;
+    for (int k = tid; k < T.nrows * 16; k += THREADS)
+      cp_async_16(dst + 4u * (uint32_t)((k >> 4) * edg::PITCH + (k & 15) * 4), g + 4 * k, pol_e);
+    const uint32_t rp = sb + edg::RP + buf * 132 * 4;
+    for (int x = tid; x <= T.rb - T.ra; x += THREADS) cp_async_4(rp + 4u * x, p.rowptr + T.ra + x);
+  };
+  // this thread's gather rows of tile T: row 64 wg + (gt >> 4) + 8 q, 16-byte piece gt & 15 (-1: past the tile's edges)
+  int sidx[8], didx[8];
+  auto load_idx = [&](const EdgeTile& T) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int r = 64 * wg + (gt >> 4) + 8 * q;
+      const bool ok = T.b >= 0 && r < T.nrows;
+      sidx[q] = ok ? __ldg(p.src + T.row0 + r) : -1;
+      didx[q] = ok ? __ldg(p.dst + T.row0 + r) : -1;
+    }
+  };
+  auto issue_proj = [&](const EdgeTile& T) {
+    if (T.b < 0) return;
+    const float* ps = p.ps + (long long)T.b * p.ps_bs + (gt & 15) * 4;
+    const float* pr = p.pr + (long long)T.b * p.pr_bs + (gt & 15) * 4;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      if (sidx[q] < 0) continue;
+      const uint32_t o = 4u * (uint32_t)((64 * wg + (gt >> 4) + 8 * q) * edg::PITCH + (gt & 15) * 4);
+      cp_async_16(sb + edg::PS + o, ps + (long long)sidx[q] * 64, pol_shared);
+      cp_async_16(sb + edg::PR + o, pr + (long long)didx[q] * 64, pol_shared);
+    }
+  };
+
+  // Every thread commits one cp.async group per issue call, empty or not, so that the groups pending at each wait are the
+  // same for all threads: the edge group of tile j + 1 is committed before tile j's GEMM 1, its projection group after it.
+  EdgeTile cur = edge_tile(p, blockIdx.x, n_work), nxt = edge_tile(p, blockIdx.x + stride, n_work);
+  load_idx(cur);
+  issue_edges(cur, 0);
+  cp_async_commit();
+  issue_proj(cur);
+  cp_async_commit();
+  load_idx(nxt);
+  float acc[32];
+  float v[2][16];
+  int buf = 0;
+  for (long long w = blockIdx.x; w < n_work; w += stride, buf ^= 1) {
+    float* stg = reinterpret_cast<float*>(s + edg::STG + buf * edg::STG_BYTES);
+    const int* rp = reinterpret_cast<const int*>(s + edg::RP + buf * 132 * 4);
+    const int nrows = cur.nrows;
+    // ---- 1. staged edge rows -> operand (TF32, zero rows past the tile's edges)
+    cp_async_wait_group<1>();  // this tile's edge group has landed (its projection group may still be in flight)
+    __syncthreads();           // ... for every thread; the previous tile's MMAs and message-buffer readers are done
+    for (int g = tid; g < 128 * 16; g += THREADS) {
+      const int i = g >> 4, c = (g & 15) * 4;
+      const float4 x = i < nrows ? *reinterpret_cast<const float4*>(stg + i * edg::PITCH + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+      *reinterpret_cast<float4*>(sA + fz_off(CH_A, i, c)) = tf32r4(x);
+    }
+    fence_proxy_async();
+    __syncthreads();
+    // ---- 2. the next tile's edge rows -> the other staging buffer, whose last readers (tile j - 1's per-receiver sums) are
+    // done.  In place (edge_out == edge) this never reads a row this CTA or another one writes: tiles are disjoint CSR
+    // edge ranges, each (batch element, tile) belongs to one CTA, and this tile's e' rows are written only after its own
+    // rows were staged.  Then the bounds of the tile after next.
+    issue_edges(nxt, buf ^ 1);
+    cp_async_commit();
+    const EdgeTile nn = edge_tile(p, w + 2 * stride, n_work);
+    // ---- 3. GEMM 1, + P_s[src] + P_r[dst], SiLU
+    fz_gemm(acc, aA, sb + edg::W1, 2);
+    const bool valid0 = rq < nrows, valid1 = rq + 8 < nrows;
+    fz_unpack(acc, v, nullptr);
+    cp_async_wait_group<1>();  // this tile's projection group has landed (the next tile's edge group may be in flight)
+    named_bar_sync(bar, 128);  // ... for the warp group that gathered (and now reads) its rows
+#pragma unroll
+    for (int a = 0; a < 2; ++a) {
+      const float* pa = a ? spr : sps;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (!(i ? valid1 : valid0)) continue;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 x = *reinterpret_cast<const float2*>(pa + (rq + 8 * i) * edg::PITCH + 8 * j + cq);
+          v[i][2 * j] += x.x;
+          v[i][2 * j + 1] += x.y;
+        }
+      }
+    }
+    named_bar_sync(bar, 128);  // the warp group's reads of the staged projections are done: gather the next tile's
+    issue_proj(nxt);
+    cp_async_commit();
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t2 = 0; t2 < 16; ++t2) v[i][t2] = silu_fast(v[i][t2]);
+    // ---- 4. GEMM 2, LayerNorm
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, aA, sb + edg::W2, 2);
+    fz_unpack(acc, v, prm);
+    fz_layernorm(v, prm + 64, prm + 128, p.eps);
+    load_idx(nn);  // the indices of the tile after next, used after the next tile's GEMM 1
+    // ---- 5. e' = e + m from the staged e rows; m over them (each thread reads, then overwrites, its own positions)
+    const int b = cur.b;
+    float* eo = p.edge_out ? p.edge_out + (long long)b * p.n_edges * 64 : nullptr;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = rq + 8 * i;
+      const long long k = (long long)cur.row0 + r;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float2* px = reinterpret_cast<float2*>(stg + r * edg::PITCH + 8 * j + cq);
+        if (eo && (i ? valid1 : valid0)) {
+          const float2 x = *px;
+          *reinterpret_cast<float2*>(eo + k * 64 + 8 * j + cq) = make_float2(x.x + v[i][2 * j], x.y + v[i][2 * j + 1]);
+        }
+        *px = make_float2(v[i][2 * j], v[i][2 * j + 1]);
+      }
+    }
+    __syncthreads();
+    // ---- 6. per-receiver sums over the tile's messages
+    const int ra = cur.ra, nrec = cur.rb - ra;
+    for (int x = tid; x < nrec * 16; x += THREADS) {
+      const int rr = x >> 4, c4 = (x & 15) * 4;
+      const int k0 = rp[rr] - cur.row0, k1 = rp[rr + 1] - cur.row0;
+      float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int k = k0; k < k1; ++k) {
+        const float4 m = *reinterpret_cast<const float4*>(stg + k * edg::PITCH + c4);
+        sum.x += m.x; sum.y += m.y; sum.z += m.z; sum.w += m.w;
+      }
+      if (p.mean) {
+        const float sc = 1.f / (float)max(k1 - k0, 1);
+        sum.x *= sc; sum.y *= sc; sum.z *= sc; sum.w *= sc;
+      }
+      *reinterpret_cast<float4*>(p.aggr + ((long long)b * p.n_rec + ra + rr) * 64 + c4) = sum;
+    }
+    cur = nxt;
+    nxt = nn;
+  }
+  cp_async_wait_group<0>();  // no copy outlives the CTA
 }
 
 // ------------------------------------------------------------------------------------ mesh -> grid decoder
@@ -1045,6 +1263,27 @@ static int fz_launch(const FzParams& p, const char* name, double bytes, cudaStre
   return NLAM_OK;
 }
 
+static int edge_split_launch(const EdgeParams& p, const char* name, double bytes, cudaStream_t st) {
+  const long long n_work = (long long)p.n_tiles * p.B;
+  if (n_work == 0) return NLAM_OK;
+  NLAM_REQUIRE(n_work < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  static unsigned mask = 0;
+  if (!(mask & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_edge_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)edg::BYTES));
+    mask |= 1u << (dev & 31);
+  }
+  const int grid = (int)std::min<long long>(n_work, num_sms());  // one CTA per SM
+  {
+    ProfScope ps(name, st, bytes);
+    tc_edge_split_kernel<<<grid, fz::THREADS, edg::BYTES, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
+}
+
 static void fz_mlp(FzParams& p, const NlamMlp* m, int k_off, int k_cols) {
   // first Linear: columns [k_off, k_off + k_cols) of w[0]; second Linear + LayerNorm
   p.w1 = wslice(m->w[0] + k_off, m->in_dim, 64, k_cols);
@@ -1229,10 +1468,7 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
                NLAM_E_INVALID, "%s: pointers / strides must be 16-byte aligned", name);
   const int Bs = (send_bs == 0 || B == 1) ? 1 : B, Br = (rec_bs == 0 || B == 1) ? 1 : B;
   const int64_t eb = B > 1 ? edge_bs : 0;
-  FzParams p;
-  memset(&p, 0, sizeof(p));
-  p.mode = fz::EDGE;
-  p.B = B;
+  const double bytes = edge_algorithmic_bytes(g, B, send_bs, rec_bs, edge_bs, edge_out != nullptr, 64);
   if (split) {
     // ws = [P_s (Bs batches) | P_r (Br batches)], computed here or (have_proj) by an earlier kernel
     float* Ps = ws;
@@ -1241,23 +1477,43 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
       int rc = fz_projections(g, em, send, send_bs, rec, rec_bs, B, Ps, Pr, st);
       if (rc) return rc;
     }
-    p.n_src = 1;
-    p.src[0] = FzSrc{edge, nullptr, eb, 64};
-    fz_mlp(p, em, 0, 64);
-    p.b1 = nullptr;  // carried by P_r
-    p.add[0] = Ps;
-    p.add_idx[0] = g->src;
-    p.add_bs[0] = Bs > 1 ? g->n_send * 64 : 0;
-    p.add[1] = Pr;
-    p.add_idx[1] = g->dst;
-    p.add_bs[1] = Br > 1 ? g->n_rec * 64 : 0;
-  } else {
-    p.n_src = 3;
-    p.src[0] = FzSrc{edge, nullptr, eb, 64};
-    p.src[1] = FzSrc{send, g->src, Bs > 1 ? send_bs : 0, 64};
-    p.src[2] = FzSrc{rec, g->dst, Br > 1 ? rec_bs : 0, 64};
-    fz_mlp(p, em, 0, 192);
+    EdgeParams q;
+    memset(&q, 0, sizeof(q));
+    q.B = B;
+    q.n_tiles = g->n_tiles;
+    q.mean = (flags & NLAM_AGGR_MEAN) ? 1 : 0;
+    q.tile_rec = g->tile_rec;
+    q.tile_edge = g->tile_edge;
+    q.rowptr = g->rowptr;
+    q.src = g->src;
+    q.dst = g->dst;
+    q.edge = edge;
+    q.edge_bs = eb;
+    q.edge_out = edge_out;
+    q.aggr = aggr_out;
+    q.ps = Ps;
+    q.pr = Pr;
+    q.ps_bs = Bs > 1 ? g->n_send * 64 : 0;
+    q.pr_bs = Br > 1 ? g->n_rec * 64 : 0;
+    q.w1 = wslice(em->w[0], em->in_dim, 64, 64);  // the edge-feature columns; b1 is carried by P_r
+    q.w2 = wslice(em->w[1], 64, em->out_dim[1], 64);
+    q.b2 = em->b[1];
+    q.gamma = em->ln_gamma;
+    q.beta = em->ln_beta;
+    q.eps = em->ln_eps;
+    q.n_rec = g->n_rec;
+    q.n_edges = g->n_edges;
+    return edge_split_launch(q, name, bytes, st);
   }
+  FzParams p;
+  memset(&p, 0, sizeof(p));
+  p.mode = fz::EDGE;
+  p.B = B;
+  p.n_src = 3;
+  p.src[0] = FzSrc{edge, nullptr, eb, 64};
+  p.src[1] = FzSrc{send, g->src, Bs > 1 ? send_bs : 0, 64};
+  p.src[2] = FzSrc{rec, g->dst, Br > 1 ? rec_bs : 0, 64};
+  fz_mlp(p, em, 0, 192);
   p.n_tiles = g->n_tiles;
   p.tile_rec = g->tile_rec;
   p.rowptr = g->rowptr;
@@ -1268,7 +1524,7 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
   p.aggr = aggr_out;
   p.n_rec = g->n_rec;
   p.n_edges = g->n_edges;
-  return fz_launch(p, name, edge_algorithmic_bytes(g, B, send_bs, rec_bs, edge_bs, edge_out != nullptr, 64), st);
+  return fz_launch(p, name, bytes, st);
 }
 
 int tc_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,

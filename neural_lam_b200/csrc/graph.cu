@@ -183,7 +183,7 @@ extern "C" int nlam_graph_create(NlamGraph** out, const int64_t* edge_index, int
   }
 
   // tensor-core tile table: whole receivers, <=kTileEdges edges and <=kTileEdges receivers
-  std::vector<int32_t> tile_rec;
+  std::vector<int32_t> tile_rec, tile_edge;
   if (maxdeg <= kTileEdges) {
     tile_rec.push_back(0);
     int64_t r = 0;
@@ -194,6 +194,7 @@ extern "C" int nlam_graph_create(NlamGraph** out, const int64_t* edge_index, int
       tile_rec.push_back((int32_t)r);
     }
     g->n_tiles = (int32_t)tile_rec.size() - 1;
+    for (int32_t r : tile_rec) tile_edge.push_back(rowptr[r]);
   }
   // uniform in-degree edge sets of degree <= 8 (mesh -> grid, mesh-down) take the uniform-degree edge path
   if (g->uniform_degree >= 1 && g->uniform_degree <= 8) g->ell_window = 1;
@@ -217,7 +218,7 @@ extern "C" int nlam_graph_create(NlamGraph** out, const int64_t* edge_index, int
   if ((rc = upload(&g->rowptr, rowptr)) || (rc = upload(&g->src, src)) || (rc = upload(&g->dst, dst)) ||
       (rc = upload(&g->perm, perm)) || (rc = upload(&g->inv_perm, inv_perm)) ||
       (rc = upload(&g->sptr, sptr)) || (rc = upload(&g->sperm, sperm)) ||
-      (rc = upload(&g->tile_rec, tile_rec))) {
+      (rc = upload(&g->tile_rec, tile_rec)) || (rc = upload(&g->tile_edge, tile_edge))) {
     cudaSetDevice(prev_dev);
     nlam_graph_destroy(g);
     return rc;
@@ -240,6 +241,7 @@ extern "C" void nlam_graph_destroy(NlamGraph* g) {
   cudaFree(g->sptr);
   cudaFree(g->sperm);
   cudaFree(g->tile_rec);
+  cudaFree(g->tile_edge);
   cudaSetDevice(prev);
   delete g;
 }
