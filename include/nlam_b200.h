@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define NLAM_ABI_VERSION 1
+#define NLAM_ABI_VERSION 2
 
 /* error codes */
 #define NLAM_OK 0
@@ -120,9 +120,8 @@ int32_t nlam_graph_max_in_degree(const NlamGraph* g);
 int32_t nlam_graph_is_sorted(const NlamGraph* g);   /* 1 if the given order already is CSR order */
 /* d if every receiver has exactly d incoming edges (mesh->grid: 4 nearest mesh nodes, reference
  * create_graph.py:779-792; mesh-down: one parent), else 0; such edge sets with update_edges=False take the
- * receiver-tiled kernels.  ell_window: 1 if additionally d <= 8 (the uniform-degree edge path applies). */
+ * receiver-tiled kernels. */
 int32_t nlam_graph_uniform_degree(const NlamGraph* g);
-int32_t nlam_graph_ell_window(const NlamGraph* g);
 /* device pointers (int32): receiver CSR, sender CSR (for gather backward), permutations */
 const int32_t* nlam_graph_rowptr(const NlamGraph* g);   /* (num_rec+1) */
 const int32_t* nlam_graph_src(const NlamGraph* g);      /* (E) sender of CSR-ordered edge k */

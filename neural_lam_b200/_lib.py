@@ -82,7 +82,6 @@ SYMBOLS = {
     "nlam_graph_max_in_degree": (ctypes.c_int32, [ctypes.c_void_p]),
     "nlam_graph_is_sorted": (ctypes.c_int32, [ctypes.c_void_p]),
     "nlam_graph_uniform_degree": (ctypes.c_int32, [ctypes.c_void_p]),
-    "nlam_graph_ell_window": (ctypes.c_int32, [ctypes.c_void_p]),
     "nlam_graph_rowptr": (ctypes.c_void_p, [ctypes.c_void_p]),
     "nlam_graph_src": (ctypes.c_void_p, [ctypes.c_void_p]),
     "nlam_graph_dst": (ctypes.c_void_p, [ctypes.c_void_p]),
@@ -218,7 +217,7 @@ def lib():
         fn = getattr(L, name)  # AttributeError if the .so is stale
         fn.restype = res
         fn.argtypes = args
-    if L.nlam_abi_version() != 1:
+    if L.nlam_abi_version() != 2:
         raise NlamError("libnlam_b200.so ABI version mismatch; rebuild")
     _lib = L
     return L

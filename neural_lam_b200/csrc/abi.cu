@@ -95,7 +95,7 @@ extern "C" int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp,
 // message buffer.
 enum InetPath { PATH_EXACT = 0, PATH_TC64 = 1, PATH_GEN = 2 };
 static size_t inet_scratch_bytes(const NlamGraph* g, int B, int H, InetPath path) {
-  if (path == PATH_TC64) return rup256(tc_edge2_workspace_floats(g, B, 0) * sizeof(float));  // node projections
+  if (path == PATH_TC64) return rup256(tc_edge_split_workspace_floats(g, B) * sizeof(float));  // node projections
   if (path == PATH_GEN) return rup256(tc_inet_gen_workspace_floats(g, B, H) * sizeof(float));
   return rup256((size_t)B * g->n_edges * H * sizeof(float));  // exact path: messages
 }
@@ -114,15 +114,13 @@ extern "C" size_t nlam_inet_workspace_bytes(const NlamGraph* g, int B, int H, in
   return rup256((size_t)B * g->n_rec * H * sizeof(float)) + need;
 }
 
-// the call shapes that take tc_edge_rmw (fused.cu) when edge_out aliases edge
+static bool labelled(const TcEdgePath& path, const char* label) { return path.label && strcmp(path.label, label) == 0; }
+
+// edge_out may alias edge where the call with edge_out = edge takes tc_edge_rmw_kernel (fused.cu, tc_edge_path)
 static bool inplace_path(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
                          int64_t rec_bs, const float* edge, int64_t edge_bs, int B, int flags) {
-  const int H = edge_mlp->out_dim[edge_mlp->n_linear - 1];
-  if (!(want_tf32(flags) && tc_edge_supported(g, edge_mlp, flags))) return false;
-  const int64_t send_rows = (B > 1 && send_bs > 0) ? send_bs / H : g->n_send;
-  if (tc_ell_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, true)) return false;
-  if (!tc_edge2_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, B, send_rows)) return false;
-  return tc_edge_rmw_supported(g, edge, edge_bs, edge, B);
+  return want_tf32(flags) &&
+         labelled(tc_edge_path(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, edge, B), "tc_edge_rmw_kernel");
 }
 
 extern "C" int nlam_inet_inplace_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs,
@@ -136,23 +134,20 @@ extern "C" int nlam_inet_inplace_supported(const NlamGraph* g, const NlamMlp* ed
 // layer's node kernel and, with next_mlp, produce those of the next layer (fused.cu)?
 static bool chain_path(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp, const NlamMlp* next_mlp,
                        const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, int B, int flags) {
-  if (!(want_tf32(flags) && tc_edge_supported(g, edge_mlp, flags)) || (flags & (NLAM_PROPAGATION | NLAM_EDGE_ONLY))) return false;
+  if (!want_tf32(flags) || (flags & (NLAM_PROPAGATION | NLAM_EDGE_ONLY))) return false;
   if (send != rec || send_bs != rec_bs || g->n_send != g->n_rec || (B > 1 && rec_bs != g->n_rec * 64)) return false;
-  if (tc_ell_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, true)) return false;
-  if (!tc_edge2_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, B, g->n_send)) return false;
+  // rule 2 of tc_edge_path: a call with an edge output takes the split form (the edge pointers only pick its label)
+  if (!tc_edge_path(g, edge_mlp, flags, send, send_bs, rec, rec_bs, rec, 0, rec, B).split) return false;
   if (next_mlp && !tc_node_proj_supported(aggr_mlp, next_mlp, rec, rec_bs, rec, g->n_rec, rec, rec)) return false;
   return true;
 }
 
-// grid -> mesh call (batch-broadcast edge features and receivers, no edge update): does nlam_inet_fwd take the split
-// tc_edge_bcast path, which can consume node projections computed by nlam_encode_fwd?
+// grid -> mesh call (batch-broadcast edge features and receivers, no edge update): does nlam_inet_fwd take
+// tc_edge_bcast_kernel, which can consume node projections computed by nlam_encode_fwd?
 static bool bcast_path(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
                        int64_t rec_bs, const float* edge, int64_t edge_bs, int B, int flags) {
-  if (!(want_tf32(flags) && tc_edge_supported(g, edge_mlp, flags))) return false;
-  const int64_t send_rows = (B > 1 && send_bs > 0) ? send_bs / 64 : g->n_send;
-  if (tc_ell_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, false)) return false;
-  if (tc_edge2_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, B, send_rows)) return false;
-  return tc_edge_bcast_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, false);
+  return want_tf32(flags) &&
+         labelled(tc_edge_path(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, nullptr, B), "tc_edge_bcast_kernel");
 }
 
 extern "C" int nlam_encode_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
@@ -298,7 +293,8 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
   const int mean = (flags & (NLAM_AGGR_MEAN | NLAM_PROPAGATION)) ? 1 : 0;  // PropagationNet forces mean
   const bool prop = flags & NLAM_PROPAGATION;
   const size_t agg_bytes = rup256((size_t)B * g->n_rec * H * sizeof(float));
-  const bool use_tc = want_tf32(flags) && tc_edge_supported(g, edge_mlp, flags);
+  const TcEdgePath path = tc_edge_path(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, B);
+  const bool use_tc = want_tf32(flags) && path.label;
   const bool use_gen = !use_tc && want_tf32(flags) &&
                        tc_inet_gen_supported(g, edge_mlp, aggr_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs);
   const size_t scratch_bytes = inet_scratch_bytes(g, B, H, use_tc ? PATH_TC64 : use_gen ? PATH_GEN : PATH_EXACT);
@@ -318,29 +314,11 @@ static int inet_fwd_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
                        scratch, st);
 
   if (use_tc) {
-    // rows of the sender tensor: known exactly when the batches are dense, else at least n_send
-    const int64_t send_rows = (B > 1 && send_bs > 0) ? send_bs / H : g->n_send;
-    int rc;
-    if (tc_ell_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge_out != nullptr)) {
-      // uniform in-degree edge sets (fused.cu)
-      rc = tc_ell_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, aggr, B, flags, st, scratch);
-    } else if (tc_edge2_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, B, send_rows)) {
-      // split first Linear: node projections + K=64 edge kernel (fused.cu)
-      // (tc_edge_rmw when the edge tensor is updated in place or not written at all)
-      // (projections computed by the previous layer's node kernel: proj_in holds [P_s | P_r] in the scratch layout)
-      float* pws = proj_in ? const_cast<float*>(proj_in) : scratch;
-      if (tc_edge_rmw_supported(g, edge, edge_bs, edge_out, B))
-        rc = tc_edge_rmw(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st, pws, proj_in != nullptr);
-      else
-        rc = tc_edge3(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st, pws, proj_in != nullptr);
-    } else if (tc_edge_bcast_supported(g, edge_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, edge_out != nullptr)) {
-      // batch-broadcast edge features and receivers, large sender set, no edge update (grid -> mesh): tile-major
-      // K = 192 kernel on raw gathered sender rows (fused.cu)
-      rc = tc_edge_bcast(g, edge_mlp, send, send_bs, rec, rec_bs, edge, aggr, B, flags, st,
-                         proj_in ? const_cast<float*>(proj_in) : scratch, proj_in != nullptr);
-    } else {
-      rc = tc_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st, send_rows);
-    }
+    // proj_in: [P_s | P_r] in the scratch layout, computed by the previous layer's node kernel or by nlam_encode_fwd
+    const bool have_proj = proj_in && path.reads_proj;
+    const int rc = path.split ? tc_edge_split(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st,
+                                              have_proj ? const_cast<float*>(proj_in) : scratch, have_proj, path.label)
+                              : tc_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr, B, flags, st);
     if (rc) return rc;
   } else {
     float* msg = scratch;

@@ -56,10 +56,6 @@ struct StepEpilogue {  // fused forecast-step epilogue of a narrow-output row ML
   const float* std;
   const float* mean;
 };
-// fused.cu: split-first-Linear edge kernel (v2) + node projection kernel
-bool tc_edge2_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
-                        const float* rec, int64_t rec_bs, int B, int64_t send_rows);
-size_t tc_edge2_workspace_floats(const NlamGraph* g, int B, int64_t send_rows_max);
 // tc7.cu: generic wgmma Linear (any K multiple of 32, N <= 256) and the layer paths built from it
 struct LinearCall {
   const float* x0;      // (B|1, n_rows, k0) rows; row pitch x0_pitch (0: dense = k0)
@@ -106,13 +102,6 @@ size_t tc_inet_gen_workspace_floats(const NlamGraph* g, int B, int H);
 int tc_inet_gen(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* aggr_mlp, const float* send, int64_t send_bs,
                 const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, float* rec_out, float* edge_out,
                 float* aggr, int B, int flags, float* ws, cudaStream_t st);
-// fused.cu: batch-broadcast edge features and receivers, no edge update (grid -> mesh)
-bool tc_edge_bcast_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
-                             const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B, bool has_edge_out);
-// (ws: [P_s | P_r] of the split form; have_proj: filled by an earlier kernel, tc_encode)
-int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
-                  bool have_proj);
 // fused.cu: the grid side of the encoder in one kernel: grid embedder on the concatenated sources, the g2m edge MLP's node
 // projections P_s (per batch element) and P_r = mesh·W1rᵀ + b1 (once), and grid_rep = grid_emb + grid_mlp(grid_emb);
 // grid_emb itself is stored where grid_emb is not NULL
@@ -127,15 +116,6 @@ bool tc_latent_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, con
                          int64_t eps_bs, const float* out, int64_t n_rows, int B, int flags);
 int tc_latent(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs, const float* eps, int64_t eps_bs,
               float* out, int64_t n_rows, int B, int flags, cudaStream_t st);
-// fused.cu: split form, out-of-place edge output
-int tc_edge3(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-             int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,
-             cudaStream_t stream, float* ws, bool have_proj = false);
-// fused.cu: same math, edge tensor updated in place or not written at all
-bool tc_edge_rmw_supported(const NlamGraph* g, const float* edge, int64_t edge_bs, const float* edge_out, int B);
-int tc_edge_rmw(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-                int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,
-                cudaStream_t stream, float* ws, bool have_proj = false);
 // fused.cu: node update of the mesh->grid layer + output_map + step epilogue in one kernel
 bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                            int64_t n_rows, int B, const float* out, const StepEpilogue* ep);
@@ -155,12 +135,6 @@ bool tc_node_proj_supported(const NlamMlp* node_mlp, const NlamMlp* next_edge_ml
                             const float* aggr, int64_t n_rows, const float* out, const float* proj_out);
 int tc_node_proj(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                  int64_t n_rows, int B, float* out, float* proj_out, cudaStream_t st);
-// fused.cu: uniform in-degree edge sets
-bool tc_ell_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
-                      const float* rec, int64_t rec_bs, bool has_edge_out);
-int tc_ell_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-                int64_t rec_bs, const float* edge, int64_t edge_bs, float* aggr_out, int B, int flags,
-                cudaStream_t stream, float* ws);
 // algorithmic bytes of the edge work of one InteractionNet call (SURVEY.md 8d without the node update)
 inline double edge_algorithmic_bytes(const NlamGraph* g, int B, int64_t send_bs, int64_t rec_bs, int64_t edge_bs, bool has_out,
                                      int H);
@@ -190,8 +164,6 @@ struct NlamGraph {
   int32_t n_tiles = 0;
   int32_t* tile_rec = nullptr;  // n_tiles+1
   int32_t* tile_edge = nullptr; // n_tiles+1: rowptr[tile_rec[t]], the first CSR edge of tile t
-  int32_t ell_window = 0;       // 1: uniform in-degree <= 8 (the uniform-degree edge path)
-  std::vector<int32_t> h_tile_rec, h_rowptr;
 };
 
 namespace nlam {
@@ -220,8 +192,21 @@ bool tc_rowmlp_supported(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, 
                          const NlamRowSrc* res2, int64_t n_rows);
 int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamRowSrc* res,
               float* out, int64_t n_rows, int B, cudaStream_t stream, const StepEpilogue* ep = nullptr);
-bool tc_edge_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags);
+// H = 64 edge stage of an InteractionNet call.  tc_edge_path decides which form and launch label the call takes (the rules
+// are listed at its definition); label NULL: the H = 64 edge kernels do not cover the call.
+struct TcEdgePath {
+  const char* label = nullptr;
+  bool split = false;       // split first Linear: node projections + K = 64 edge GEMM (tc_edge_split); else K = 192 (tc_edge)
+  bool reads_proj = false;  // the split form can take projections an earlier kernel computed (proj_in) instead of its own pass
+};
+TcEdgePath tc_edge_path(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
+                        const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, const float* edge_out, int B);
+// ws: [P_s | P_r], tc_edge_split_workspace_floats floats; have_proj: filled by an earlier kernel (tc_node_proj, tc_encode)
+size_t tc_edge_split_workspace_floats(const NlamGraph* g, int B);
+int tc_edge_split(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
+                  int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,
+                  cudaStream_t stream, float* ws, bool have_proj, const char* label);
 int tc_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs,
             const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out,
-            float* aggr_out, int B, int flags, cudaStream_t stream, int64_t send_rows);
+            float* aggr_out, int B, int flags, cudaStream_t stream);
 }  // namespace nlam

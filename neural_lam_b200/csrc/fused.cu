@@ -15,10 +15,11 @@
 // tc_rowlinear_kernel (node projections P_s = x_s·W1sᵀ, P_r = x_r·W1rᵀ + b1 of the split first edge Linear, both node
 // sets in one grid), tc_edge_kernel (K = 192 edge MLP on raw gathered rows), tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
 // epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).  The split-form edge stage
-// (first edge Linear split into e·W1eᵀ and node projections gathered in its epilogue) runs in tc_edge_split_kernel below,
-// under the labels tc_edge3_kernel (out-of-place edge output), tc_edge_rmw_kernel (edge tensor updated in place or not
-// written), tc_ell_window_kernel (uniform in-degree edge sets) and tc_edge_bcast_kernel (batch-broadcast edge features
-// and receivers).
+// (first edge Linear split into e·W1eᵀ and node projections gathered in its epilogue) runs in tc_edge_split_kernel below
+// (tc_edge_split).  tc_edge_path decides, in one place, whether an edge stage takes the split or the K = 192 form and under
+// which label the split kernel is launched: tc_edge3_kernel (out-of-place edge output), tc_edge_rmw_kernel (edge tensor
+// updated in place or not written), tc_ell_window_kernel (uniform in-degree edge sets) or tc_edge_bcast_kernel
+// (batch-broadcast edge features and receivers).
 #include "tc_ptx.cuh"
 #include "wgmma_tf32.cuh"
 
@@ -1399,7 +1400,7 @@ static int fz_projections(const NlamGraph* g, const NlamMlp* em, const float* se
 }
 
 // ---- edge stage: messages, optional edge output, per-receiver aggregate
-bool tc_edge_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags) {
+static bool tc_edge_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags) {
   int nout = 0;
   if (flags & NLAM_PROPAGATION) return false;
   if (!g || g->n_tiles <= 0) return false;
@@ -1408,7 +1409,7 @@ bool tc_edge_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags) {
 }
 
 static int edge_mode_env() {
-  // NLAM_TC_EDGE=v1 | v2 forces one formulation of the first edge Linear
+  // NLAM_TC_EDGE=v1 | v2 forces one formulation of the first edge Linear (rule 2 of tc_edge_path)
   static int mode = -1;
   if (mode < 0) {
     const char* e = getenv("NLAM_TC_EDGE");
@@ -1417,45 +1418,38 @@ static int edge_mode_env() {
   return mode;
 }
 
-bool tc_edge2_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
-                        const float* rec, int64_t rec_bs, int B, int64_t send_rows) {
-  (void)send_rows;
-  // default: the split form (node projections + K = 64 edge GEMM) where the per-node projection pass is small next to the
-  // edge work (mesh graph: ~9 edges per node); the K = 192 form otherwise (grid -> mesh)
+// Which form and launch label an edge stage takes: the first rule that applies (DESIGN.md §4.1).  The split form and the
+// K = 192 form round differently in TF32, and only tc_edge_rmw_kernel may write its edge output over its edge input, so the
+// dispatch and every support query in abi.cu ask here.
+//   1. no edge output, uniform in-degree 1..8: split, tc_ell_window_kernel, always with its own projection pass
+//   2. NLAM_TC_EDGE=v2, or (unless v1) E·B >= 2.5·(n_send·Bs + n_rec·Br): the projection pass is small next to the edge
+//      work (mesh graphs): split, tc_edge_rmw_kernel without edge output or with it over a dense edge input, else
+//      tc_edge3_kernel
+//   3. no edge output, edge features and receivers shared by the batch (grid -> mesh): split, tc_edge_bcast_kernel; both
+//      projections are far fewer rows than the batch's edges
+//   4. otherwise: K = 192 on raw gathered rows, tc_edge_kernel
+// Rules 1 and 2 need send / rec 16-byte aligned and both batch strides % 4 == 0, rule 3 send / rec / edge aligned and
+// send_bs % 4 == 0.  Bs (Br) is 1 for senders (receivers) shared by the batch, else B.
+TcEdgePath tc_edge_path(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
+                        const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, const float* edge_out, int B) {
+  if (!tc_edge_supported(g, edge_mlp, flags)) return {};
+  const bool aligned = aligned16(send) && aligned16(rec) && send_bs % 4 == 0 && rec_bs % 4 == 0;
+  if (!edge_out && g->uniform_degree >= 1 && g->uniform_degree <= 8 && aligned) return {"tc_ell_window_kernel", true, false};
   const int mode = edge_mode_env();
-  if (mode == 1) return false;
-  if (!tc_edge_supported(g, edge_mlp, flags)) return false;
-  if (!(aligned16(send) && aligned16(rec) && send_bs % 4 == 0 && rec_bs % 4 == 0)) return false;
-  if (mode == 2) return true;
   const double edge_rows = (double)g->n_edges * B;
   const double node_rows = (double)g->n_send * ((send_bs == 0 || B == 1) ? 1 : B) +
                            (double)g->n_rec * ((rec_bs == 0 || B == 1) ? 1 : B);
-  return edge_rows >= 2.5 * node_rows;
+  if (aligned && (mode == 2 || (mode != 1 && edge_rows >= 2.5 * node_rows))) {
+    const bool rmw = !edge_out || (edge_out == edge && (B == 1 || edge_bs == g->n_edges * 64));
+    return {rmw ? "tc_edge_rmw_kernel" : "tc_edge3_kernel", true, true};
+  }
+  if (!edge_out && (edge_bs == 0 || B == 1) && (rec_bs == 0 || B == 1) && aligned16(send) && aligned16(rec) && aligned16(edge) &&
+      send_bs % 4 == 0)
+    return {"tc_edge_bcast_kernel", true, true};
+  return {"tc_edge_kernel", false, false};
 }
 
-size_t tc_edge2_workspace_floats(const NlamGraph* g, int B, int64_t send_rows_max) {
-  (void)send_rows_max;
-  return (size_t)B * (size_t)(g->n_send + g->n_rec) * 64 + 64;
-}
-
-bool tc_edge_bcast_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
-                             const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs, int B, bool has_edge_out) {
-  if (has_edge_out || !tc_edge_supported(g, edge_mlp, flags)) return false;
-  if (!(edge_bs == 0 || B == 1) || !(rec_bs == 0 || B == 1)) return false;  // edge features and receivers shared by the batch
-  return aligned16(send) && aligned16(rec) && aligned16(edge) && send_bs % 4 == 0;
-}
-
-bool tc_ell_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, const float* send, int64_t send_bs,
-                      const float* rec, int64_t rec_bs, bool has_edge_out) {
-  if (has_edge_out || !g || g->uniform_degree < 1 || g->uniform_degree > 8 || !g->ell_window) return false;
-  if (!tc_edge_supported(g, edge_mlp, flags)) return false;
-  return aligned16(send) && aligned16(rec) && send_bs % 4 == 0 && rec_bs % 4 == 0;
-}
-
-bool tc_edge_rmw_supported(const NlamGraph* g, const float* edge, int64_t edge_bs, const float* edge_out, int B) {
-  if (!edge_out) return true;
-  return edge_out == edge && (B == 1 || edge_bs == (int64_t)g->n_edges * 64);
-}
+size_t tc_edge_split_workspace_floats(const NlamGraph* g, int B) { return (size_t)B * (size_t)(g->n_send + g->n_rec) * 64 + 64; }
 
 // split: A = e, + P_s[src] + P_r[dst] in the GEMM 1 epilogue (projections in ws, or from the previous layer when have_proj);
 // otherwise A = [e | x_src | x_dst] (K = 192)
@@ -1527,42 +1521,17 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
   return fz_launch(p, name, bytes, st);
 }
 
+int tc_edge_split(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
+                  int64_t rec_bs, const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags,
+                  cudaStream_t st, float* ws, bool have_proj, const char* label) {
+  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, ws, true, have_proj,
+                 label);
+}
+
 int tc_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
-            const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st,
-            int64_t send_rows) {
-  (void)send_rows;
+            const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st) {
   return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, nullptr, false, false,
                  "tc_edge_kernel");
-}
-
-int tc_edge3(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
-             const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
-             bool have_proj) {
-  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, ws, true, have_proj,
-                 "tc_edge3_kernel");
-}
-
-int tc_edge_rmw(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
-                const float* edge, int64_t edge_bs, float* edge_out, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
-                bool have_proj) {
-  NLAM_REQUIRE(!edge_out || edge_out == edge, NLAM_E_INVALID, "tc_edge_rmw: the edge output must alias the edge input");
-  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, edge_out, aggr_out, B, flags, st, ws, true, have_proj,
-                 "tc_edge_rmw_kernel");
-}
-
-int tc_ell_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec, int64_t rec_bs,
-                const float* edge, int64_t edge_bs, float* aggr_out, int B, int flags, cudaStream_t st, float* ws) {
-  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, nullptr, aggr_out, B, flags, st, ws, true, false,
-                 "tc_ell_window_kernel");
-}
-
-int tc_edge_bcast(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int64_t send_bs, const float* rec,
-                  int64_t rec_bs, const float* edge, float* aggr_out, int B, int flags, cudaStream_t st, float* ws,
-                  bool have_proj) {
-  // split form: the batch-shared receiver projection is computed once, the sender projection once per node (both far fewer
-  // rows than the batch's edges), and the edge GEMM has K = 64 instead of gathering K = 192 raw rows per edge and batch
-  return fz_edge(g, edge_mlp, send, send_bs, rec, rec_bs, edge, 0, nullptr, aggr_out, B, flags, st, ws, true, have_proj,
-                 "tc_edge_bcast_kernel");
 }
 
 // ---- node update chained with the next layer's projections / with output_map + step epilogue

@@ -113,7 +113,7 @@ extern "C" int nlam_abi_version(void) { return NLAM_ABI_VERSION; }
 extern "C" const char* nlam_last_error(void) { return nlam::get_error(); }
 extern "C" int64_t nlam_launch_count(void) { return nlam::launch_count(); }
 extern "C" const char* nlam_build_info(void) {
-  return "libnlam_b200 abi=1 arch=sm_90a cuda=" __DATE__;
+  return "libnlam_b200 abi=2 arch=sm_90a cuda=" __DATE__;
 }
 
 template <class T>
@@ -196,10 +196,6 @@ extern "C" int nlam_graph_create(NlamGraph** out, const int64_t* edge_index, int
     g->n_tiles = (int32_t)tile_rec.size() - 1;
     for (int32_t r : tile_rec) tile_edge.push_back(rowptr[r]);
   }
-  // uniform in-degree edge sets of degree <= 8 (mesh -> grid, mesh-down) take the uniform-degree edge path
-  if (g->uniform_degree >= 1 && g->uniform_degree <= 8) g->ell_window = 1;
-  g->h_tile_rec = tile_rec;
-  g->h_rowptr = rowptr;
 
   int prev_dev = 0;
   cudaError_t e = cudaGetDevice(&prev_dev);
@@ -252,7 +248,6 @@ extern "C" int64_t nlam_graph_num_send(const NlamGraph* g) { return g->n_send; }
 extern "C" int32_t nlam_graph_max_in_degree(const NlamGraph* g) { return g->max_in_degree; }
 extern "C" int32_t nlam_graph_is_sorted(const NlamGraph* g) { return g->is_sorted; }
 extern "C" int32_t nlam_graph_uniform_degree(const NlamGraph* g) { return g->uniform_degree; }
-extern "C" int32_t nlam_graph_ell_window(const NlamGraph* g) { return g->ell_window; }
 extern "C" const int32_t* nlam_graph_rowptr(const NlamGraph* g) { return g->rowptr; }
 extern "C" const int32_t* nlam_graph_src(const NlamGraph* g) { return g->src; }
 extern "C" const int32_t* nlam_graph_dst(const NlamGraph* g) { return g->dst; }

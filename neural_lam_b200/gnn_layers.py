@@ -16,11 +16,6 @@ from . import _lib, backward, ops
 from .networks import _aten_forward, make_mlp
 
 _DEFAULT_MATH = "auto"
-# in-place edge update of the middle layers of a no-grad stack (csrc/fused.cu: each tile writes e + m over its own edge rows); the
-# library decides per call shape (nlam_inet_inplace_supported), other shapes stay out of place
-_INPLACE_EDGE_UPDATE = True
-# the node kernel of a stacked layer also computes the next layer's node projections (csrc/fused.cu)
-_CHAIN_PROJECTIONS = True
 _MATH_FLAGS = {"auto": 0, "tf32": _lib.MATH_TF32, "fp32": _lib.MATH_FP32}
 
 
@@ -355,9 +350,10 @@ class InteractionNet(nn.Module):
         _, (s3, r3, e3) = self._batchify(node_rep, node_rep, edge_rep)
         g = self._graph(r3.device)
         write_edges = keep_edges or not last
-        inplace = _INPLACE_EDGE_UPDATE and (not first) and write_edges and e3.is_contiguous()
+        # in place where the library supports the call shape (nlam_inet_inplace_supported), else out of place
+        inplace = (not first) and write_edges and e3.is_contiguous()
         nxt = None
-        if (_CHAIN_PROJECTIONS and next_layer is not None and isinstance(next_layer, InteractionNet) and next_layer._stackable()
+        if (next_layer is not None and isinstance(next_layer, InteractionNet) and next_layer._stackable()
                 and self._stackable() and next_layer.num_rec == self.num_rec and r3.shape[0] > 0):
             fl = self._flags()
             if (ops.inet_chain_supported(g, self.edge_mlp, self.aggr_mlp, next_layer.edge_mlp, r3, fl)

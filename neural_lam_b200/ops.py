@@ -202,7 +202,6 @@ class Graph:
         self.max_in_degree = L.nlam_graph_max_in_degree(h)
         self.is_sorted = bool(L.nlam_graph_is_sorted(h))
         self.uniform_degree = L.nlam_graph_uniform_degree(h)
-        self.ell_window = L.nlam_graph_ell_window(h)
         self.perm = L.nlam_graph_perm(h)
         self.inv_perm = L.nlam_graph_inv_perm(h)
 
