@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define NLAM_ABI_VERSION 2
+#define NLAM_ABI_VERSION 3
 
 /* error codes */
 #define NLAM_OK 0
@@ -204,36 +204,25 @@ int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
  * and once for the batch P_r = mesh·W1rᵀ + b1 (W1r = columns 128..191; mesh (g2m receivers, 64) shared by the batch).
  * grid_rep (B, n_rows, 64) dense; proj = [P_s (B, n_rows, 64) | P_r (n_rec, 64)], 16-byte aligned: the proj_in of the g2m call
  * nlam_inet_fwd_chain(g2m, ..., send = P_s, rec = mesh, edge = g2m_edge, next_edge_mlp = NULL, proj_in = proj), whose edge
- * stage then skips its own projection pass.  Covered: TF32 math, H = 64, every MLP in -> 64 -> 64 with biases and an affine
- * LayerNorm, g2m senders = the n_rows grid rows, and a g2m call that takes the batch-broadcast split edge path (edge features
- * and mesh rows shared by the batch); nlam_encode_supported says whether a call is.  NLAM_E_UNSUPPORTED otherwise (callers
- * then run nlam_rowmlp_fwd for the embedder, nlam_inet_fwd for g2m and nlam_rowmlp_fwd for grid_mlp). */
+ * stage then skips its own projection pass.  Two optional extras, not both in one call (NLAM_E_INVALID):
+ *   - g2m_edge_mlp_b with proj_b: a second grid -> mesh layer on the same grid embedding, receivers and edge features (the
+ *     hierarchical Graph-EFM's prior and decoder g2m layers, reference latent/hi_graph_encoder.py:148-150,
+ *     hi_graph_decoder.py:216-218); proj_b = [P_s_b (B, n_rows, 64) | P_r_b (n_rec, 64)] of g2m_edge_mlp_b, 16-byte aligned,
+ *     is the proj_in of that layer's call (send = P_s_b);
+ *   - grid_emb: grid_emb itself is stored (B, n_rows, 64) dense, 16-byte aligned; Graph-EFM's decoder reads it as the senders
+ *     of its grid -> mesh layer (reference latent/base_decoder.py:145-155).
+ * Covered: TF32 math, H = 64, every MLP in -> 64 -> 64 with biases and an affine LayerNorm, g2m senders = the n_rows grid
+ * rows, and g2m calls that take the batch-broadcast split edge path (edge features and mesh rows shared by the batch);
+ * nlam_encode_supported says whether a call is.  NLAM_E_UNSUPPORTED otherwise (callers then run nlam_rowmlp_fwd for the
+ * embedder, nlam_inet_fwd for each g2m layer and nlam_rowmlp_fwd for grid_mlp). */
 int nlam_encode_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
-                          const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge,
-                          int64_t edge_bstride, const float* grid_rep, const float* proj, int64_t n_rows, int B, int flags);
+                          const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b, const float* mesh, int64_t mesh_bstride,
+                          const float* g2m_edge, int64_t edge_bstride, const float* grid_rep, const float* proj,
+                          const float* proj_b, const float* grid_emb, int64_t n_rows, int B, int flags);
 int nlam_encode_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
-                    const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge, int64_t edge_bstride,
-                    float* grid_rep, float* proj, int64_t n_rows, int B, int flags, void* stream);
-/* nlam_encode_fwd that also stores grid_emb (B, n_rows, 64) dense, 16-byte aligned: Graph-EFM's decoder reads it as the
- * senders of its grid -> mesh layer (reference latent/base_decoder.py:145-155).  Same coverage as nlam_encode_fwd. */
-int nlam_encode_emb_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
-                        const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bstride, const float* g2m_edge,
-                        int64_t edge_bstride, float* grid_rep, float* proj, float* grid_emb, int64_t n_rows, int B, int flags,
-                        void* stream);
-/* nlam_encode_fwd for two grid -> mesh layers on the same grid embedding, receivers and edge features (the hierarchical
- * Graph-EFM's prior and decoder g2m layers, reference latent/hi_graph_encoder.py:148-150, hi_graph_decoder.py:216-218): the
- * launch also computes proj_b = [P_s_b (B, n_rows, 64) | P_r_b (n_rec, 64)] of g2m_edge_mlp_b, the proj_in of the second
- * layer's nlam_inet_fwd_chain call (send = P_s_b).  grid_emb is not stored.  Covered where nlam_encode_fwd covers the first
- * layer and the second layer's call takes the same batch-broadcast split edge path; nlam_encode2_supported says whether a
- * call is.  NLAM_E_UNSUPPORTED otherwise. */
-int nlam_encode2_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
-                           const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b, const float* mesh,
-                           int64_t mesh_bstride, const float* g2m_edge, int64_t edge_bstride, const float* grid_rep,
-                           const float* proj, const float* proj_b, int64_t n_rows, int B, int flags);
-int nlam_encode2_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const NlamMlp* grid_mlp,
-                     const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b, const float* mesh, int64_t mesh_bstride,
-                     const float* g2m_edge, int64_t edge_bstride, float* grid_rep, float* proj, float* proj_b, int64_t n_rows,
-                     int B, int flags, void* stream);
+                    const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b, const float* mesh, int64_t mesh_bstride,
+                    const float* g2m_edge, int64_t edge_bstride, float* grid_rep, float* proj, float* proj_b, float* grid_emb,
+                    int64_t n_rows, int B, int flags, void* stream);
 /* The stochastic step of Graph-EFM (reference latent/graph_encoder.py:102-105, base_encoder.py:85-94,
  * base_decoder.py:145) in one launch (csrc/fused.cu).  Per row r of batch element b, x (B, n_rows, 64) the prior's mesh
  * representation and eps (B, n_rows, 64) standard normal noise, both with dense rows and batch strides x_bstride /

@@ -151,70 +151,41 @@ static bool bcast_path(const NlamGraph* g, const NlamMlp* edge_mlp, const float*
 }
 
 extern "C" int nlam_encode_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
-                                     const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bs,
-                                     const float* g2m_edge, int64_t edge_bs, const float* grid_rep, const float* proj,
+                                     const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b,
+                                     const float* mesh, int64_t mesh_bs, const float* g2m_edge, int64_t edge_bs,
+                                     const float* grid_rep, const float* proj, const float* proj_b, const float* grid_emb,
                                      int64_t n_rows, int B, int flags) {
   if (!g2m || !embed_mlp || !srcs || !grid_mlp || !g2m_edge_mlp || !mesh || !g2m_edge || !grid_rep || !proj) return 0;
-  if (B < 1 || g2m->n_send != n_rows || (B > 1 && mesh_bs != 0) || (((uintptr_t)grid_rep | (uintptr_t)proj) & 15)) return 0;
-  if (!tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags)) return 0;
-  // the g2m call that consumes the projections: send = P_s, dense (B, n_rows, 64) at the start of proj
-  return bcast_path(g2m, g2m_edge_mlp, proj, B > 1 ? n_rows * 64 : 0, mesh, mesh_bs, g2m_edge, edge_bs, B, flags) ? 1 : 0;
+  if (!g2m_edge_mlp_b != !proj_b || (g2m_edge_mlp_b && grid_emb)) return 0;
+  if (B < 1 || g2m->n_send != n_rows || (B > 1 && mesh_bs != 0) ||
+      (((uintptr_t)grid_rep | (uintptr_t)proj | (uintptr_t)proj_b) & 15))
+    return 0;
+  // each g2m call that consumes its projections: send = its P_s, dense (B, n_rows, 64) at the start of its proj
+  const NlamMlp* edge_mlps[2] = {g2m_edge_mlp, g2m_edge_mlp_b};
+  const float* projs[2] = {proj, proj_b};
+  for (int i = 0; i < 2 && edge_mlps[i]; ++i) {
+    if (!tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, edge_mlps[i], mesh, g2m->n_rec, n_rows, B, flags)) return 0;
+    if (!bcast_path(g2m, edge_mlps[i], projs[i], B > 1 ? n_rows * 64 : 0, mesh, mesh_bs, g2m_edge, edge_bs, B, flags)) return 0;
+  }
+  return 1;
 }
 
 extern "C" int nlam_encode_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
-                               const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bs,
-                               const float* g2m_edge, int64_t edge_bs, float* grid_rep, float* proj, int64_t n_rows, int B,
-                               int flags, void* stream) {
+                               const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b,
+                               const float* mesh, int64_t mesh_bs, const float* g2m_edge, int64_t edge_bs, float* grid_rep,
+                               float* proj, float* proj_b, float* grid_emb, int64_t n_rows, int B, int flags, void* stream) {
   NLAM_REQUIRE(g2m && embed_mlp && srcs && grid_mlp && g2m_edge_mlp && mesh && g2m_edge && grid_rep && proj, NLAM_E_INVALID,
                "nlam_encode_fwd: null argument");
-  NLAM_REQUIRE(nlam_encode_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, mesh_bs, g2m_edge, edge_bs,
-                                     grid_rep, proj, n_rows, B, flags),
+  NLAM_REQUIRE(!g2m_edge_mlp_b == !proj_b, NLAM_E_INVALID, "nlam_encode_fwd: g2m_edge_mlp_b and proj_b go together");
+  NLAM_REQUIRE(!(g2m_edge_mlp_b && grid_emb), NLAM_E_INVALID, "nlam_encode_fwd: grid_emb is not stored with a second g2m edge MLP");
+  NLAM_REQUIRE(((uintptr_t)grid_emb & 15) == 0, NLAM_E_INVALID, "nlam_encode_fwd: unaligned grid_emb");
+  NLAM_REQUIRE(nlam_encode_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, g2m_edge_mlp_b, mesh, mesh_bs, g2m_edge,
+                                     edge_bs, grid_rep, proj, proj_b, grid_emb, n_rows, B, flags),
                NLAM_E_UNSUPPORTED, "nlam_encode_fwd: graph / shape / math mode not covered by the fused encoder");
-  return tc_encode(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags, grid_rep, proj,
-                   proj + (size_t)B * n_rows * 64, nullptr, (cudaStream_t)stream);
-}
-
-extern "C" int nlam_encode_emb_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
-                                   const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const float* mesh, int64_t mesh_bs,
-                                   const float* g2m_edge, int64_t edge_bs, float* grid_rep, float* proj, float* grid_emb,
-                                   int64_t n_rows, int B, int flags, void* stream) {
-  NLAM_REQUIRE(g2m && embed_mlp && srcs && grid_mlp && g2m_edge_mlp && mesh && g2m_edge && grid_rep && proj && grid_emb,
-               NLAM_E_INVALID, "nlam_encode_emb_fwd: null argument");
-  NLAM_REQUIRE(((uintptr_t)grid_emb & 15) == 0, NLAM_E_INVALID, "nlam_encode_emb_fwd: unaligned grid_emb");
-  NLAM_REQUIRE(nlam_encode_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, mesh_bs, g2m_edge, edge_bs,
-                                     grid_rep, proj, n_rows, B, flags),
-               NLAM_E_UNSUPPORTED, "nlam_encode_emb_fwd: graph / shape / math mode not covered by the fused encoder");
-  return tc_encode(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags, grid_rep, proj,
-                   proj + (size_t)B * n_rows * 64, grid_emb, (cudaStream_t)stream);
-}
-
-extern "C" int nlam_encode2_supported(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
-                                      const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b,
-                                      const float* mesh, int64_t mesh_bs, const float* g2m_edge, int64_t edge_bs,
-                                      const float* grid_rep, const float* proj, const float* proj_b, int64_t n_rows, int B,
-                                      int flags) {
-  if (!g2m_edge_mlp_b || !proj_b || ((uintptr_t)proj_b & 15)) return 0;
-  if (!nlam_encode_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, mesh_bs, g2m_edge, edge_bs, grid_rep,
-                             proj, n_rows, B, flags))
-    return 0;
-  if (!tc_encode_supported(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp_b, mesh, g2m->n_rec, n_rows, B, flags)) return 0;
-  // the second g2m call consumes its projections on the same path as the first
-  return bcast_path(g2m, g2m_edge_mlp_b, proj_b, B > 1 ? n_rows * 64 : 0, mesh, mesh_bs, g2m_edge, edge_bs, B, flags) ? 1 : 0;
-}
-
-extern "C" int nlam_encode2_fwd(const NlamGraph* g2m, const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src,
-                                const NlamMlp* grid_mlp, const NlamMlp* g2m_edge_mlp, const NlamMlp* g2m_edge_mlp_b,
-                                const float* mesh, int64_t mesh_bs, const float* g2m_edge, int64_t edge_bs, float* grid_rep,
-                                float* proj, float* proj_b, int64_t n_rows, int B, int flags, void* stream) {
-  NLAM_REQUIRE(g2m && embed_mlp && srcs && grid_mlp && g2m_edge_mlp && g2m_edge_mlp_b && mesh && g2m_edge && grid_rep && proj &&
-                   proj_b,
-               NLAM_E_INVALID, "nlam_encode2_fwd: null argument");
-  NLAM_REQUIRE(nlam_encode2_supported(g2m, embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, g2m_edge_mlp_b, mesh, mesh_bs,
-                                      g2m_edge, edge_bs, grid_rep, proj, proj_b, n_rows, B, flags),
-               NLAM_E_UNSUPPORTED, "nlam_encode2_fwd: graph / shape / math mode not covered by the fused encoder");
   const size_t grid_floats = (size_t)B * n_rows * 64;
   return tc_encode(embed_mlp, srcs, n_src, grid_mlp, g2m_edge_mlp, mesh, g2m->n_rec, n_rows, B, flags, grid_rep, proj,
-                   proj + grid_floats, nullptr, (cudaStream_t)stream, g2m_edge_mlp_b, proj_b, proj_b + grid_floats);
+                   proj + grid_floats, grid_emb, (cudaStream_t)stream, g2m_edge_mlp_b, proj_b,
+                   proj_b ? proj_b + grid_floats : nullptr);
 }
 
 extern "C" int nlam_latent_sample_supported(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x, int64_t x_bs,

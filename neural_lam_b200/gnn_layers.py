@@ -391,41 +391,31 @@ class InteractionNet(nn.Module):
     @torch.no_grad()
     def encode_step(self, embedder, grid_mlp, grid_inputs, rec_rep, edge_rep, want_grid_emb=False, second=None):
         """Inference-only, for the grid -> mesh layer of a forecast step: ``grid_emb = embedder(cat grid_inputs)``, this layer's
-        node projections and ``grid_rep = grid_emb + grid_mlp(grid_emb)`` in one launch (``ops.encode``; grid_emb never goes
-        to HBM), then this layer's edge stage on those projections and its node update.  Returns ``(rec_rep', grid_rep)``, or
-        None when the layer / graph / call shape has no such path (the caller then runs the three calls).
-        ``want_grid_emb``: the launch also stores grid_emb, returned third (Graph-EFM's decoder reads it).
-        ``second``: another grid -> mesh layer on the same graph, receivers and edge features, with grid_emb as its senders
-        (the hierarchical Graph-EFM's decoder g2m): the launch also computes its projections, and its output is returned
-        third; grid_emb is not stored."""
-        if not self._edge_stage_separable():
-            return None
-        if second is not None and not (second._edge_stage_separable() and self._same_edges(second)):
+        node projections and ``grid_rep = grid_emb + grid_mlp(grid_emb)`` in one launch (``ops.encode``), then this layer's
+        edge stage on those projections and its node update.  ``second``: another grid -> mesh layer on the same graph,
+        receivers and edge features, with grid_emb as its senders (the hierarchical Graph-EFM's decoder g2m): the launch also
+        computes its projections.  ``want_grid_emb``: the launch also stores grid_emb (Graph-EFM's decoder reads it; not with
+        ``second``).  Returns ``(grid_rep, [rec_rep' of this layer (, of second)], grid_emb | None)``, or None when the layer /
+        graph / call shape has no such path (the caller then runs the embedder, the layers and grid_mlp as separate calls)."""
+        layers = [self] if second is None else [self, second]
+        if not all(layer._edge_stage_separable() for layer in layers) or (second is not None and not self._same_edges(second)):
             return None
         _, (r3, e3) = self._batchify(rec_rep, edge_rep)
         if r3.shape[-2] != self.num_rec or e3.shape[-2] != self.num_edges or r3.device != self._src32.device:
             return None
-        g = self._graph(r3.device)
-        fl = self._flags() | embedder.nlam_flags | grid_mlp.nlam_flags
-        if second is not None:
-            fl |= second._flags()
-        enc = ops.encode(g, embedder, grid_inputs, grid_mlp, self.edge_mlp, r3, e3, flags=fl, want_emb=want_grid_emb,
-                         edge_seq_b=second.edge_mlp if second is not None else None)
+        fl = embedder.nlam_flags | grid_mlp.nlam_flags
+        for layer in layers:
+            fl |= layer._flags()
+        enc = ops.encode(self._graph(r3.device), embedder, grid_inputs, grid_mlp, self.edge_mlp, r3, e3, flags=fl,
+                         want_emb=want_grid_emb, edge_seq_b=second.edge_mlp if second is not None else None)
         if enc is None:
             return None
-        grid_rep = enc[0]
+        grid_rep, projs, grid_emb = enc
         B, G = grid_rep.shape[0], grid_rep.shape[1]
-        outs = []
-        for layer, proj in ((self, enc[1]), (second, enc[2] if second is not None else None)):
-            if layer is None:
-                continue
-            ps = proj[: B * G * 64].view(B, G, 64)
-            rec_out, _, _, _ = ops.inet_fwd(layer._graph(r3.device), layer.edge_mlp, layer.aggr_mlp, ps, r3.expand(B, -1, -1),
-                                            e3.expand(B, -1, -1), False, layer._flags(), proj_in=proj)
-            outs.append(rec_out)
-        if second is not None:
-            return outs[0], grid_rep, outs[1]
-        return (outs[0], grid_rep, enc[2]) if want_grid_emb else (outs[0], grid_rep)
+        outs = [ops.inet_fwd(layer._graph(r3.device), layer.edge_mlp, layer.aggr_mlp, proj[: B * G * 64].view(B, G, 64),
+                             r3.expand(B, -1, -1), e3.expand(B, -1, -1), False, layer._flags(), proj_in=proj)[0]
+                for layer, proj in zip(layers, projs)]
+        return grid_rep, outs, grid_emb
 
     def _same_edges(self, other):
         """Does ``other`` have this layer's edge set?  Compared once per pair (outside any CUDA-graph capture: the first

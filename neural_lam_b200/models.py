@@ -66,6 +66,23 @@ class BufferList(nn.Module):
         return (getattr(self, f"b{i}") for i in range(self.n))
 
 
+def _encode_grid(embedder, grid_mlp, sources, mesh, g2m_emb, layers, want_grid_emb=False):
+    """The grid side of a step's encoder: ``grid_emb = embedder(cat sources)``, the grid -> mesh ``layers`` (zero, one or two,
+    each with grid_emb as senders, ``mesh`` as receivers and ``g2m_emb`` as edge features) and ``grid_rep = grid_emb +
+    grid_mlp(grid_emb)`` -> ``(grid_rep, [each layer's mesh representation], grid_emb if want_grid_emb else None)``.
+    Without grad, one launch computes the embedder, the layers' node projections and grid_mlp where the library covers the
+    shapes (``InteractionNet.encode_step``); else the calls are composed."""
+    if layers and not torch.is_grad_enabled():
+        enc = layers[0].encode_step(embedder, grid_mlp, sources, mesh, g2m_emb, want_grid_emb=want_grid_emb,
+                                    second=layers[1] if len(layers) > 1 else None)
+        if enc is not None:
+            return enc
+    grid_emb = embedder.apply_rows(sources)
+    mesh_reps = [layer(grid_emb, mesh, g2m_emb) for layer in layers]
+    grid_rep = grid_mlp.apply_rows([grid_emb], res=grid_emb)  # graph/base.py:308-310
+    return grid_rep, mesh_reps, grid_emb if want_grid_emb else None
+
+
 class StepPredictor(nn.Module):
     """One-step predictor ``(X_{t-1}, X_t, forcing_t) -> X_{t+1}`` (reference
     models/step_predictors/base.py)."""
@@ -215,21 +232,12 @@ class BaseGraphModel(StepPredictor):
         """Grid embedder, grid -> mesh layer and encoding grid MLP (reference graph/base.py:275-310) ->
         (static embeddings, mesh_rep, grid_rep)."""
         B = prev_state.shape[0]
+        st = self.static_embeddings()
         # grid feature concat (base.py:275-283) is fused into the embedder kernel
         sources = [prev_state, prev_prev_state, forcing, self.expand_to_batch(self.grid_static_features, B)]
-        if not torch.is_grad_enabled():
-            # one launch for the embedder, the g2m node projections and the encoding grid MLP where the library covers the
-            # shapes; the grid embedding never goes to HBM.  forward_with_boundary and the no-grad forward both take it, so the
-            # eager and the captured step compute the same values
-            st = self.static_embeddings()
-            fused = self.g2m_gnn.encode_step(self.grid_embedder, self.encoding_grid_mlp, sources,
-                                             self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
-            if fused is not None:
-                return st, fused[0], fused[1]
-        grid_emb = self.grid_embedder.apply_rows(sources)
-        st = self.static_embeddings()
-        mesh_rep = self.g2m_gnn(grid_emb, self.expand_to_batch(st["mesh_emb"], B), self.expand_to_batch(st["g2m_emb"], B))
-        grid_rep = self.encoding_grid_mlp.apply_rows([grid_emb], res=grid_emb)  # base.py:308-310
+        grid_rep, (mesh_rep,), _ = _encode_grid(self.grid_embedder, self.encoding_grid_mlp, sources,
+                                                self.expand_to_batch(st["mesh_emb"], B),
+                                                self.expand_to_batch(st["g2m_emb"], B), [self.g2m_gnn])
         return st, mesh_rep, grid_rep
 
     def forward(self, prev_state, prev_prev_state, forcing):
@@ -239,31 +247,15 @@ class BaseGraphModel(StepPredictor):
         st, mesh_rep, grid_rep = self._encode(prev_state, prev_prev_state, forcing)
         mesh_rep = self.process_step(mesh_rep, st)
         m2g_emb = self.expand_to_batch(st["m2g_emb"], B)
-        inference = not torch.is_grad_enabled() and not self.output_std and not self.clamps_output
-        if inference and hasattr(self.m2g_gnn, "decode_step"):
-            # the fused decoder, as forward_with_boundary runs it: the eager and the captured step compute the same values
-            fused = self.m2g_gnn.decode_step(mesh_rep, grid_rep, m2g_emb, self.output_map, prev_state, None, None, self.diff_std,
-                                             self.diff_mean, out_flags=self.output_map.nlam_flags)
-            if fused is not None:
-                return fused, None
-        grid_rep = self.m2g_gnn(mesh_rep, grid_rep, m2g_emb)
-        if inference:
-            # output_map + rescale (base.py:339) + residual (base.py:342) in one launch where the library fuses it
-            fused = ops.rowmlp_step(self.output_map, grid_rep, prev_state, None, None, self.diff_std, self.diff_mean,
-                                    flags=self.output_map.nlam_flags)
-            if fused is not None:
-                return fused, None
-        net_output = self.output_map(grid_rep)
+        if not torch.is_grad_enabled():
+            # the decoder forward_with_boundary runs: the eager and the captured step launch the same kernels
+            return self._decode(self.m2g_gnn, self.output_map, mesh_rep, grid_rep, m2g_emb, prev_state, None, None)
+        net_output = self.output_map(self.m2g_gnn(mesh_rep, grid_rep, m2g_emb))
         if self.output_std:
             pred_delta_mean, pred_std_raw = net_output.chunk(2, dim=-1)
             pred_std = torch.nn.functional.softplus(pred_std_raw)
         else:
             pred_delta_mean, pred_std = net_output, None
-        if not torch.is_grad_enabled():
-            # rescale (base.py:339) + (clamped) residual update (base.py:342, step_predictors/base.py:366-396) in one kernel
-            clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
-            return ops.step_epilogue(pred_delta_mean.contiguous(), prev_state, None, None, self.diff_std, self.diff_mean,
-                                     clamp=clamp), pred_std
         rescaled = pred_delta_mean * self.diff_std + self.diff_mean
         return self.get_clamped_new_state(rescaled, prev_state), pred_std
 
@@ -275,39 +267,46 @@ class BaseGraphModel(StepPredictor):
         B = prev_state.shape[0]
         st, mesh_rep, grid_rep = self._encode(prev_state, prev_prev_state, forcing)
         mesh_rep = self.process_step(mesh_rep, st)
+        return self._decode(self.m2g_gnn, self.output_map, mesh_rep, grid_rep, self.expand_to_batch(st["m2g_emb"], B), prev_state,
+                            boundary_state, boundary_mask, out)[0]
+
+    def _decode(self, m2g, out_map, mesh_rep, grid_rep, m2g_emb, prev_state, boundary, bmask, out=None):
+        """The no-grad decoder: the mesh -> grid layer ``m2g``, the output MLP ``out_map``, the rescale and (clamped) residual
+        update (graph/base.py:322-342, step_predictors/base.py:366-396) and the boundary mix (autoregressive.py:128-131;
+        ``boundary`` None: none) -> (new_state, pred_std|None).  The first of these that covers the call runs:
+          1. ``m2g.decode_step``: all of it in two launches (the m2g graph has a uniform in-degree the kernel covers);
+          2. ``m2g.aggregate_only``, then the node update, ``out_map`` and the step epilogue in one launch
+             (``ops.node_update_step``): the updated grid representation never goes to HBM;
+          3. the m2g layer, then ``out_map`` and the step epilogue in one launch (``ops.rowmlp_step``);
+          4. the m2g layer, ``out_map`` and ``ops.step_epilogue``: the one rung for clamped outputs and a predicted std."""
         clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
-        m2g_emb = self.expand_to_batch(st["m2g_emb"], B)
-        if clamp is None and hasattr(self.m2g_gnn, "aggregate_only"):
-            # the whole decoder (edge projections, then edges + aggregation + node update + output_map + step epilogue in one
-            # kernel) where the m2g graph has a uniform in-degree the kernel covers
-            fused = self.m2g_gnn.decode_step(mesh_rep, grid_rep, m2g_emb, self.output_map, prev_state, boundary_state,
-                                             boundary_mask, self.diff_std, self.diff_mean,
-                                             out_flags=self.output_map.nlam_flags, out=out)
+        if clamp is None and not self.output_std:
+            fused = m2g.decode_step(mesh_rep, grid_rep, m2g_emb, out_map, prev_state, boundary, bmask, self.diff_std,
+                                    self.diff_mean, out_flags=out_map.nlam_flags, out=out)
             if fused is not None:
-                return fused
-            # node update of the mesh->grid layer + output_map + step epilogue in one kernel: the updated grid
-            # representation (which nothing else reads) never goes to HBM
-            aggr = self.m2g_gnn.aggregate_only(mesh_rep, grid_rep, m2g_emb)
+                return fused, None
+            aggr = m2g.aggregate_only(mesh_rep, grid_rep, m2g_emb)
             if aggr is not None:
-                fused = ops.node_update_step(self.m2g_gnn.aggr_mlp, self.output_map, grid_rep, aggr, prev_state, boundary_state,
-                                             boundary_mask, self.diff_std, self.diff_mean,
-                                             flags=self.output_map.nlam_flags, out=out)
+                fused = ops.node_update_step(m2g.aggr_mlp, out_map, grid_rep, aggr, prev_state, boundary, bmask, self.diff_std,
+                                             self.diff_mean, flags=out_map.nlam_flags, out=out)
                 if fused is not None:
-                    return fused
-                grid_rep = self.m2g_gnn._kernel_node_update(grid_rep, aggr)
+                    return fused, None
+                grid_rep = m2g._kernel_node_update(grid_rep, aggr)
             else:
-                grid_rep = self.m2g_gnn(mesh_rep, grid_rep, m2g_emb)
-        else:
-            grid_rep = self.m2g_gnn(mesh_rep, grid_rep, m2g_emb)
-        if clamp is None:
-            fused = ops.rowmlp_step(self.output_map, grid_rep, prev_state, boundary_state, boundary_mask, self.diff_std,
-                                    self.diff_mean, flags=self.output_map.nlam_flags, out=out)
+                grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
+            fused = ops.rowmlp_step(out_map, grid_rep, prev_state, boundary, bmask, self.diff_std, self.diff_mean,
+                                    flags=out_map.nlam_flags, out=out)
             if fused is not None:
-                return fused
-        net_output = self.output_map(grid_rep)
-        # rescale + (clamped) update + boundary mix in one kernel
-        return ops.step_epilogue(net_output, prev_state, boundary_state, boundary_mask, self.diff_std, self.diff_mean,
-                                 out=out, clamp=clamp)
+                return fused, None
+        else:
+            grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
+        net_output = out_map(grid_rep)
+        pred_std = None
+        if self.output_std:
+            net_output, std_raw = net_output.chunk(2, dim=-1)
+            pred_std = torch.nn.functional.softplus(std_raw)
+        return ops.step_epilogue(net_output, prev_state, boundary, bmask, self.diff_std, self.diff_mean, out=out,
+                                 clamp=clamp), pred_std
 
 
 class GraphLAM(BaseGraphModel):
@@ -654,40 +653,6 @@ class BaseGraphEFM(BaseGraphModel):
         mean, std = prior.mean_std(dist)
         return dec.latent_embedder.apply_rows([mean + eps * std])
 
-    def _decode(self, mesh_rep, grid_rep, m2g_emb, prev_state, boundary, bmask, out):
-        """m2g + param_map + (clamped) step epilogue with the boundary mix: the fused decoder where the graph / shapes allow,
-        else the launch chains ``BaseGraphModel.forward_with_boundary`` falls back to -> (new_state, pred_std|None)."""
-        dec = self.decoder
-        m2g, pm = dec.m2g_gnn, dec.param_map
-        clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
-        if clamp is None and not self.output_std:
-            fused = m2g.decode_step(mesh_rep, grid_rep, m2g_emb, pm, prev_state, boundary, bmask, self.diff_std, self.diff_mean,
-                                    out_flags=pm.nlam_flags, out=out)
-            if fused is not None:
-                return fused, None
-            aggr = m2g.aggregate_only(mesh_rep, grid_rep, m2g_emb)
-            if aggr is not None:
-                fused = ops.node_update_step(m2g.aggr_mlp, pm, grid_rep, aggr, prev_state, boundary, bmask, self.diff_std,
-                                             self.diff_mean, flags=pm.nlam_flags, out=out)
-                if fused is not None:
-                    return fused, None
-                grid_rep = m2g._kernel_node_update(grid_rep, aggr)
-            else:
-                grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
-            fused = ops.rowmlp_step(pm, grid_rep, prev_state, boundary, bmask, self.diff_std, self.diff_mean,
-                                    flags=pm.nlam_flags, out=out)
-            if fused is not None:
-                return fused, None
-        else:
-            grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
-        net_output = pm(grid_rep)
-        pred_std = None
-        if self.output_std:
-            net_output, std_raw = net_output.chunk(2, dim=-1)
-            pred_std = torch.nn.functional.softplus(std_raw)
-        return ops.step_epilogue(net_output.contiguous(), prev_state, boundary, bmask, self.diff_std, self.diff_mean, out=out,
-                                 clamp=clamp), pred_std
-
 
 class GraphEFMMultiScale(BaseGraphEFM):
     """Graph-EFM on a flat (multiscale) mesh (reference step_predictors/graph/graph_efm.py: GraphEFMMultiScale :796-1037):
@@ -758,22 +723,13 @@ class GraphEFMMultiScale(BaseGraphEFM):
         prior, dec = self.prior_model, self.decoder
         learned = isinstance(prior, GraphLatentEncoder)
         sources = self._grid_sources(prev_state, prev_prev_state, forcing)
-        enc = None
-        if learned:
-            enc = prior.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, ge["mesh"], ge["g2m"],
-                                            want_grid_emb=True)
-        if enc is not None:
-            mesh_rep, res_grid, grid_emb = enc
-        else:
-            grid_emb = self.grid_prev_embedder.apply_rows(sources)
-            res_grid = dec.grid_update_mlp.apply_rows([grid_emb], res=grid_emb)
-            mesh_rep = prior.g2m_gnn(grid_emb, ge["mesh"], ge["g2m"]) if learned else None
+        res_grid, prior_reps, grid_emb = _encode_grid(self.grid_prev_embedder, dec.grid_update_mlp, sources, ge["mesh"],
+                                                      ge["g2m"], [prior.g2m_gnn] if learned else [], want_grid_emb=True)
         eps = self._noise(latent_noise, B, prev_state.device)
-        if learned:
-            mesh_rep = prior.process_mesh(mesh_rep, ge["m2m"])
+        mesh_rep = prior.process_mesh(prior_reps[0], ge["m2m"]) if learned else None
         latent_emb = self._sample_latent(mesh_rep, grid_emb, eps)
         mesh_rep = dec.mesh_step(grid_emb, latent_emb, ge)
-        return self._decode(mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+        return self._decode(dec.m2g_gnn, dec.param_map, mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
 
 
 class GraphEFM(BaseGraphEFM):
@@ -868,30 +824,14 @@ class GraphEFM(BaseGraphEFM):
         prior, dec = self.prior_model, self.decoder
         learned = isinstance(prior, HiGraphLatentEncoder)
         sources = self._grid_sources(prev_state, prev_prev_state, forcing)
-        mesh0, g2m = ge["mesh"][0], ge["g2m"]
-        grid_emb = prior_rep = None
-        if learned:
-            enc = prior.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0, g2m,
-                                            second=dec.g2m_gnn)
-            if enc is not None:
-                prior_rep, res_grid, dec_rep = enc
-        else:
-            enc = dec.g2m_gnn.encode_step(self.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0, g2m)
-            if enc is not None:
-                dec_rep, res_grid = enc
-        if enc is None:
-            grid_emb = self.grid_prev_embedder.apply_rows(sources)
-            res_grid = dec.grid_update_mlp.apply_rows([grid_emb], res=grid_emb)
-            prior_rep = prior.g2m_gnn(grid_emb, mesh0, g2m) if learned else None
-            dec_rep = dec.g2m_gnn(grid_emb, mesh0, g2m)
+        res_grid, reps, _ = _encode_grid(self.grid_prev_embedder, dec.grid_update_mlp, sources, ge["mesh"][0], ge["g2m"],
+                                         [prior.g2m_gnn, dec.g2m_gnn] if learned else [dec.g2m_gnn])
         eps = self._noise(latent_noise, B, prev_state.device)
-        if learned:
-            prior_rep = prior.process_mesh(prior_rep, ge)
-        elif grid_emb is None:  # the constant prior reads only the batch size and device of its input
-            grid_emb = res_grid
-        latent_emb = self._sample_latent(prior_rep, grid_emb, eps)
-        mesh_rep = dec.mesh_step(dec_rep, latent_emb, ge)
-        return self._decode(mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+        prior_rep = prior.process_mesh(reps[0], ge) if learned else None
+        # the constant prior reads only the batch size and device of its input: res_grid stands in for the grid embedding
+        latent_emb = self._sample_latent(prior_rep, res_grid, eps)
+        mesh_rep = dec.mesh_step(reps[-1], latent_emb, ge)
+        return self._decode(dec.m2g_gnn, dec.param_map, mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
 
 
 MODELS = {"graph_lam": GraphLAM, "hi_lam": HiLAM, "hi_lam_parallel": HiLAMParallel}

@@ -96,21 +96,41 @@ def mlp_struct(seq):
     return s
 
 
-def _src(t, bs, dim, idx=None):
-    r = NlamRowSrc()
-    r.ptr = t.data_ptr()
-    r.idx = idx
-    r.bstride = bs
-    r.dim = dim
-    return r
-
-
 def _iptr(t, offset_rows=0):
     """Device address of an int32 index tensor (offset by whole entries)."""
     if t is None:
         return None
     assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous()
     return t.data_ptr() + 4 * offset_rows
+
+
+def _row_srcs(prepared, idx=None, r0=0):
+    """NlamRowSrc array of ``as_rows`` views ``(t, B, batch stride)``: row r of source i reads row r0 + r of it, or the row
+    ``idx[i][r0 + r]`` where ``idx[i]`` (an int32 device tensor) is given."""
+    arr = (NlamRowSrc * len(prepared))()
+    for r, (t, _, bs), ix in zip(arr, prepared, idx or [None] * len(prepared)):
+        d = t.shape[-1]
+        r.ptr, r.idx = (t.data_ptr() + 4 * r0 * d, None) if ix is None else (t.data_ptr(), _iptr(ix, r0))
+        r.bstride, r.dim = bs, d
+    return arr
+
+
+def _step_io(prev, boundary, bmask, out):
+    """The forecast-step epilogue's tensors: ``prev`` (B, G, D), ``boundary`` of prev's shape with its (G) mask ``bmask`` (or
+    both None), ``out`` of prev's shape, not prev itself (allocated when None) -> the four, contiguous."""
+    prev = prev.contiguous()
+    if boundary is not None:
+        assert bmask is not None, "a boundary state needs its mask"
+        boundary, bmask = boundary.contiguous(), bmask.contiguous()
+        assert boundary.shape == prev.shape and bmask.numel() == prev.shape[1]
+    if out is None:
+        out = torch.empty_like(prev)
+    assert out.is_contiguous() and out.shape == prev.shape and out.data_ptr() != prev.data_ptr()
+    return prev, boundary, bmask, out
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
 
 
 def rowmlp(seq, sources, res=None, flags=0, idx=None, res_idx=None, row_range=None):
@@ -135,40 +155,20 @@ def rowmlp(seq, sources, res=None, flags=0, idx=None, res_idx=None, row_range=No
     r0, r1 = (0, n_total) if row_range is None else row_range
     n_rows = r1 - r0
     dev = prepared[0][0].device
-    arr = (NlamRowSrc * len(prepared))()
-    for i, ((t, b, bs), ix) in enumerate(zip(prepared, idx)):
-        if b not in (1, B):
-            raise ValueError("rowmlp: sources disagree on batch size")
-        d = t.shape[-1]
-        if ix is None:
-            arr[i].ptr = t.data_ptr() + 4 * r0 * d
-            arr[i].idx = None
-        else:
-            arr[i].ptr = t.data_ptr()
-            arr[i].idx = _iptr(ix, r0)
-        arr[i].bstride = bs
-        arr[i].dim = d
+    if any(b not in (1, B) for _, b, _ in prepared):
+        raise ValueError("rowmlp: sources disagree on batch size")
+    arr = _row_srcs(prepared, idx, r0)
     mlp = mlp_struct(seq)
     nf = mlp.out_dim[mlp.n_linear - 1]
     three_d = any(s.dim() == 3 for s in sources) or (res is not None and res.dim() == 3)
     resp = None
-    keep = None
     if res is not None:
         keep, rb, rbs = as_rows(res)
         _require_cuda(keep)
         if rb not in (1, B) and B != 1:
             raise ValueError("rowmlp: residual batch mismatch")
         B = max(B, rb)
-        rs = NlamRowSrc()
-        if res_idx is None:
-            rs.ptr = keep.data_ptr() + 4 * r0 * nf
-            rs.idx = None
-        else:
-            rs.ptr = keep.data_ptr()
-            rs.idx = _iptr(res_idx, r0)
-        rs.bstride = rbs
-        rs.dim = nf
-        resp = ctypes.pointer(rs)
+        resp = _row_srcs([(keep, rb, rbs)], [res_idx], r0)
     out = torch.empty((B, n_rows, nf), device=dev, dtype=torch.float32)
     with torch.cuda.device(dev):
         _lib.check(L.nlam_rowmlp_fwd(ctypes.byref(mlp), arr, len(prepared), resp, None, out.data_ptr(), None,
@@ -372,29 +372,22 @@ def step_epilogue(net_out, prev, boundary, bmask, diff_std, diff_mean, out=None,
     (kind int32 (D), lo (D), up (D)): the clamped update of models/step_predictors/base.py:366-396 instead of the plain
     residual for the variables with limits."""
     L = _lib.lib()
-    net_out, prev = net_out.contiguous(), prev.contiguous()
+    net_out = net_out.contiguous()
     _require_cuda(net_out, prev, diff_std, diff_mean, boundary, bmask)
     B, G, D = net_out.shape
     if prev.shape != net_out.shape or diff_std.numel() != D or diff_mean.numel() != D:
         raise ValueError(f"step_epilogue: net_out {tuple(net_out.shape)}, prev {tuple(prev.shape)}, diff statistics "
                          f"{diff_std.numel()}/{diff_mean.numel()} disagree")
-    if out is None:
-        out = torch.empty_like(net_out)
-    assert out.is_contiguous() and out.shape == net_out.shape
-    if boundary is not None:
-        boundary, bmask = boundary.contiguous(), bmask.contiguous()
-        assert bmask.numel() == G
+    prev, boundary, bmask, out = _step_io(prev, boundary, bmask, out)
     with torch.cuda.device(net_out.device):
-        bp = boundary.data_ptr() if boundary is not None else None
-        mp = bmask.data_ptr() if boundary is not None else None
         if clamp is not None:
             kind, lo, up = clamp
             assert kind.dtype == torch.int32 and kind.numel() == D and lo.numel() == D and up.numel() == D
-            _lib.check(L.nlam_step_epilogue_clamped(net_out.data_ptr(), prev.data_ptr(), bp, mp, diff_std.data_ptr(),
-                                                    diff_mean.data_ptr(), kind.data_ptr(), lo.data_ptr(), up.data_ptr(),
-                                                    out.data_ptr(), B, G, D, _stream_ptr(net_out.device)))
+            _lib.check(L.nlam_step_epilogue_clamped(net_out.data_ptr(), prev.data_ptr(), _ptr(boundary), _ptr(bmask),
+                                                    diff_std.data_ptr(), diff_mean.data_ptr(), kind.data_ptr(), lo.data_ptr(),
+                                                    up.data_ptr(), out.data_ptr(), B, G, D, _stream_ptr(net_out.device)))
         else:
-            _lib.check(L.nlam_step_epilogue(net_out.data_ptr(), prev.data_ptr(), bp, mp, diff_std.data_ptr(),
+            _lib.check(L.nlam_step_epilogue(net_out.data_ptr(), prev.data_ptr(), _ptr(boundary), _ptr(bmask), diff_std.data_ptr(),
                                             diff_mean.data_ptr(), out.data_ptr(), B, G, D, _stream_ptr(net_out.device)))
     return out
 
@@ -407,28 +400,14 @@ def rowmlp_step(seq, x, prev, boundary, bmask, diff_std, diff_mean, flags=0, out
     if flags & _lib.MATH_FP32:
         return None
     xr, B, bs = as_rows(x)
-    prev = prev.contiguous()
     _require_cuda(xr, prev, diff_std, diff_mean, boundary, bmask)
     mlp = mlp_struct(seq)
-    D = mlp.out_dim[mlp.n_linear - 1]
     G = xr.shape[-2]
-    if D >= 64 or mlp.ln_gamma or prev.shape != (B, G, D):
+    if prev.shape != (B, G, mlp.out_dim[mlp.n_linear - 1]):
         return None
-    arr = (NlamRowSrc * 1)()
-    arr[0].ptr = xr.data_ptr()
-    arr[0].idx = None
-    arr[0].bstride = bs
-    arr[0].dim = xr.shape[-1]
-    if boundary is not None:
-        boundary, bmask = boundary.contiguous(), bmask.contiguous()
-        assert boundary.shape == prev.shape and bmask.numel() == G
-    if out is None:
-        out = torch.empty_like(prev)
-    assert out.is_contiguous() and out.shape == prev.shape and out.data_ptr() != prev.data_ptr()
+    prev, boundary, bmask, out = _step_io(prev, boundary, bmask, out)
     with torch.cuda.device(xr.device):
-        rc = L.nlam_rowmlp_step_fwd(ctypes.byref(mlp), arr, 1, prev.data_ptr(),
-                                    boundary.data_ptr() if boundary is not None else None,
-                                    bmask.data_ptr() if boundary is not None else None,
+        rc = L.nlam_rowmlp_step_fwd(ctypes.byref(mlp), _row_srcs([(xr, B, bs)]), 1, prev.data_ptr(), _ptr(boundary), _ptr(bmask),
                                     diff_std.data_ptr(), diff_mean.data_ptr(), out.data_ptr(), G, B, flags,
                                     _stream_ptr(xr.device))
     if rc == _lib.E_UNSUPPORTED:
@@ -446,25 +425,18 @@ def node_update_step(node_seq, out_seq, rec, aggr, prev, boundary, bmask, diff_s
         return None
     rr, B, rbs = as_rows(rec)
     ar, Ba, abs_ = as_rows(aggr)
-    prev = prev.contiguous()
     _require_cuda(rr, ar, prev, diff_std, diff_mean, boundary, bmask)
     nm, om = mlp_struct(node_seq), mlp_struct(out_seq)
     D = om.out_dim[om.n_linear - 1]
     G = rr.shape[-2]
     Bt = max(B, Ba)
-    if (rr.shape[-1] != 64 or ar.shape[-1] != 64 or ar.shape[-2] != G or D >= 64 or om.ln_gamma or prev.shape != (Bt, G, D)
-            or Ba != Bt or (Bt > 1 and abs_ != G * 64) or B not in (1, Bt)):
+    if (rr.shape[-1] != 64 or ar.shape[-1] != 64 or ar.shape[-2] != G or prev.shape != (Bt, G, D) or Ba != Bt
+            or (Bt > 1 and abs_ != G * 64) or B not in (1, Bt)):
         return None
-    if boundary is not None:
-        boundary, bmask = boundary.contiguous(), bmask.contiguous()
-        assert boundary.shape == prev.shape and bmask.numel() == G
-    if out is None:
-        out = torch.empty_like(prev)
-    assert out.is_contiguous() and out.shape == prev.shape and out.data_ptr() != prev.data_ptr()
+    prev, boundary, bmask, out = _step_io(prev, boundary, bmask, out)
     with torch.cuda.device(rr.device):
         rc = L.nlam_node_update_step_fwd(ctypes.byref(nm), ctypes.byref(om), rr.data_ptr(), rbs if B > 1 else 0, ar.data_ptr(),
-                                         prev.data_ptr(), boundary.data_ptr() if boundary is not None else None,
-                                         bmask.data_ptr() if boundary is not None else None, diff_std.data_ptr(),
+                                         prev.data_ptr(), _ptr(boundary), _ptr(bmask), diff_std.data_ptr(),
                                          diff_mean.data_ptr(), out.data_ptr(), G, Bt, flags, _stream_ptr(rr.device))
     if rc == _lib.E_UNSUPPORTED:
         return None
@@ -485,7 +457,6 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
     s, Bs, sbs = as_rows(send)
     r, Br, rbs = as_rows(rec)
     e, Be, ebs = as_rows(edge_csr)
-    prev = prev.contiguous()
     _require_cuda(s, r, e, prev, diff_std, diff_mean, boundary, bmask)
     B = max(Bs, Br, Be)
     em, nm, om = mlp_struct(edge_seq), mlp_struct(node_seq), mlp_struct(out_seq)
@@ -495,21 +466,14 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
             or e.shape[-1] != 64 or G != graph.n_rec or s.shape[-2] < graph.n_send or e.shape[-2] != graph.n_edges
             or prev.shape != (B, G, D) or r.device != graph.device):
         return None
-    if boundary is not None:
-        assert bmask is not None, "decode_step: a boundary state needs its mask"
-        boundary, bmask = boundary.contiguous(), bmask.contiguous()
-        assert boundary.shape == prev.shape and bmask.numel() == G
-    if out is None:
-        out = torch.empty_like(prev)
-    assert out.is_contiguous() and out.shape == prev.shape and out.data_ptr() != prev.data_ptr()
+    prev, boundary, bmask, out = _step_io(prev, boundary, bmask, out)
     dev = r.device
     ws_bytes = L.nlam_decode_workspace_bytes(graph.handle, B)
     ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
     with torch.cuda.device(dev):
         rc = L.nlam_decode_step_fwd(graph.handle, ctypes.byref(em), ctypes.byref(nm), ctypes.byref(om),
                                     s.data_ptr(), sbs if Bs > 1 else 0, r.data_ptr(), rbs if Br > 1 else 0, e.data_ptr(),
-                                    ebs if Be > 1 else 0, prev.data_ptr(), boundary.data_ptr() if boundary is not None else None,
-                                    bmask.data_ptr() if boundary is not None else None, diff_std.data_ptr(),
+                                    ebs if Be > 1 else 0, prev.data_ptr(), _ptr(boundary), _ptr(bmask), diff_std.data_ptr(),
                                     diff_mean.data_ptr(), out.data_ptr(), B, flags, ws.data_ptr(), ws_bytes, _stream_ptr(dev))
     if rc == _lib.E_UNSUPPORTED:
         return None
@@ -519,18 +483,16 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
 
 def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=0, want_emb=False, edge_seq_b=None):
     """The grid side of a forecast step's encoder in ONE launch (``nlam_encode_fwd``): ``grid_emb = embed_seq(cat sources)``
-    stays on chip; returns ``(grid_rep, proj)`` with ``grid_rep = grid_emb + grid_seq(grid_emb)`` (B, G, 64) and
-    ``proj = [P_s | P_r]`` flat, ``P_s = grid_emb·W1sᵀ`` (B, G, 64) and ``P_r = mesh·W1rᵀ + b1`` (n_mesh, 64) of the grid -> mesh
-    layer's edge MLP ``edge_seq`` on ``graph`` — the ``proj_in`` of that layer's ``inet_fwd`` with send = P_s.  ``mesh`` and
-    ``edge_csr`` are shared by the batch.  ``want_emb``: also store grid_emb (``nlam_encode_emb_fwd``) and return
-    ``(grid_rep, proj, grid_emb)``.  ``edge_seq_b``: the edge MLP of a second grid -> mesh layer on the same graph, receivers
-    and edge features (``nlam_encode2_fwd``); returns ``(grid_rep, proj, proj_b)`` with that layer's projections.  Returns
-    None when the library does not fuse these shapes / this math mode (the caller then runs the embedder, the g2m layer(s)
-    and ``grid_seq`` as separate calls)."""
+    and ``grid_rep = grid_emb + grid_seq(grid_emb)`` (B, G, 64), and for the grid -> mesh layer on ``graph`` whose edge MLP is
+    ``edge_seq`` (and for a second one, ``edge_seq_b``, on the same graph; both with grid_emb as senders, ``mesh`` as
+    receivers and ``edge_csr`` as edge features, shared by the batch) ``proj = [P_s | P_r]`` flat, ``P_s = grid_emb·W1sᵀ``
+    (B, G, 64) and ``P_r = mesh·W1rᵀ + b1`` (n_mesh, 64) — the ``proj_in`` of that layer's ``inet_fwd`` with send = P_s.
+    Returns ``(grid_rep, [proj per layer], grid_emb | None)``; grid_emb is stored where ``want_emb`` (not with
+    ``edge_seq_b``), else it stays on chip.  Returns None when the library does not fuse these shapes / this math mode (the
+    caller then runs the embedder, the g2m layer(s) and ``grid_seq`` as separate calls)."""
     L = _lib.lib()
     if flags & _lib.MATH_FP32:
         return None
-    assert not (want_emb and edge_seq_b is not None), "encode: grid_emb is not stored with a second edge MLP"
     prepared = [as_rows(t) for t in sources]
     m, Bm, mbs = as_rows(mesh)
     e, Be, ebs = as_rows(edge_csr)
@@ -541,35 +503,22 @@ def encode(graph, embed_seq, sources, grid_seq, edge_seq, mesh, edge_csr, flags=
             or Bm not in (1, B) or Be not in (1, B) or m.shape[-1] != 64 or e.shape[-1] != 64
             or m.shape[-2] != graph.n_rec or e.shape[-2] != graph.n_edges or m.device != graph.device):
         return None
-    arr = (NlamRowSrc * len(prepared))()
-    for i, (t, _, bs) in enumerate(prepared):
-        arr[i].ptr = t.data_ptr()
-        arr[i].idx = None
-        arr[i].bstride = bs
-        arr[i].dim = t.shape[-1]
-    em, gm, sm = mlp_struct(embed_seq), mlp_struct(grid_seq), mlp_struct(edge_seq)
+    edge_seqs = [edge_seq] if edge_seq_b is None else [edge_seq, edge_seq_b]
+    second = edge_seq_b is not None
+    em, gm = mlp_struct(embed_seq), mlp_struct(grid_seq)
+    sm = [mlp_struct(s) for s in edge_seqs]
     grid_rep = torch.empty((B, G, 64), device=m.device, dtype=torch.float32)
-    proj = torch.empty((B * G + graph.n_rec) * 64, device=m.device, dtype=torch.float32)
-    args = (m.data_ptr(), mbs if Bm > 1 else 0, e.data_ptr(), ebs if Be > 1 else 0, grid_rep.data_ptr(), proj.data_ptr())
+    projs = [torch.empty((B * G + graph.n_rec) * 64, device=m.device, dtype=torch.float32) for _ in edge_seqs]
     grid_emb = torch.empty((B, G, 64), device=m.device, dtype=torch.float32) if want_emb else None
     with torch.cuda.device(m.device):
-        if edge_seq_b is not None:
-            sm_b = mlp_struct(edge_seq_b)
-            proj_b = torch.empty_like(proj)
-            rc = L.nlam_encode2_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
-                                    ctypes.byref(sm_b), *args, proj_b.data_ptr(), G, B, flags, _stream_ptr(m.device))
-        elif want_emb:
-            rc = L.nlam_encode_emb_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
-                                       *args, grid_emb.data_ptr(), G, B, flags, _stream_ptr(m.device))
-        else:
-            rc = L.nlam_encode_fwd(graph.handle, ctypes.byref(em), arr, len(prepared), ctypes.byref(gm), ctypes.byref(sm),
-                                   *args, G, B, flags, _stream_ptr(m.device))
+        rc = L.nlam_encode_fwd(graph.handle, ctypes.byref(em), _row_srcs(prepared), len(prepared), ctypes.byref(gm),
+                               ctypes.byref(sm[0]), ctypes.byref(sm[1]) if second else None, m.data_ptr(), mbs if Bm > 1 else 0,
+                               e.data_ptr(), ebs if Be > 1 else 0, grid_rep.data_ptr(), projs[0].data_ptr(),
+                               projs[1].data_ptr() if second else None, _ptr(grid_emb), G, B, flags, _stream_ptr(m.device))
     if rc == _lib.E_UNSUPPORTED:
         return None
     _lib.check(rc)
-    if edge_seq_b is not None:
-        return grid_rep, proj, proj_b
-    return (grid_rep, proj, grid_emb) if want_emb else (grid_rep, proj)
+    return grid_rep, projs, grid_emb
 
 
 def latent_sample(param_seq, embed_seq, x, eps, flags=0):

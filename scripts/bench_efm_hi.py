@@ -99,13 +99,14 @@ def main():
 
     @torch.no_grad()
     def two_g2m():
-        out["two_g2m"] = prior_g2m.encode_step(m.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0, g2m,
-                                               second=dec.g2m_gnn)
+        grid_rep, (prior_rep, dec_rep), _ = prior_g2m.encode_step(m.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0,
+                                                                  g2m, second=dec.g2m_gnn)
+        out["two_g2m"] = (prior_rep, grid_rep, dec_rep)
 
     @torch.no_grad()
     def emit_emb():
-        prior_rep, grid_rep, grid_emb = prior_g2m.encode_step(m.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0, g2m,
-                                                              want_grid_emb=True)
+        grid_rep, (prior_rep,), grid_emb = prior_g2m.encode_step(m.grid_prev_embedder, dec.grid_update_mlp, sources, mesh0,
+                                                                 g2m, want_grid_emb=True)
         out["emit_emb"] = (prior_rep, grid_rep, dec.g2m_gnn(grid_emb, mesh0, g2m))
 
     launches = {}

@@ -86,7 +86,7 @@ def main():
     def edge_only_with_proj():
         # the same edge stage on the fused projections: its time is subtracted from old() so that both sides time the
         # three launches the kernel replaces
-        ps = state["fused"][1]
+        ps = state["fused"][1][0]
         _lib.check(L.nlam_inet_fwd_chain(g.handle, ctypes.byref(em), ctypes.byref(am), None, ps.data_ptr(), G * 64,
                                          mesh.data_ptr(), 0, g2m.data_ptr(), 0, None, None, aggr.data_ptr(), ps.data_ptr(),
                                          None, B, flags | _lib.EDGE_ONLY, ws.data_ptr(), ws_bytes, ops._stream_ptr(dev)))
@@ -115,7 +115,7 @@ def main():
     old()
     fused()
     torch.cuda.synchronize()
-    grid_rep, proj = state["fused"]
+    grid_rep, (proj,), _ = state["fused"]
     n_ps = B * G * 64
     diff = max((grid_rep - state["old"]).abs().max().item(),
                (proj[:n_ps] - proj_old[:n_ps]).abs().max().item(),

@@ -19,7 +19,7 @@ def _declared_symbols():
     return sorted(set(re.findall(r"\b(nlam_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_library_loads_at_abi_version_2_and_exports_every_declared_symbol():
+def test_library_loads_at_abi_version_3_and_exports_every_declared_symbol():
     L = ctypes.CDLL(_lib.LIB_PATH)
     names = _declared_symbols()
     assert len(names) >= 20
@@ -27,7 +27,7 @@ def test_library_loads_at_abi_version_2_and_exports_every_declared_symbol():
         assert hasattr(L, n), f"{n} declared in include/nlam_b200.h but not exported"
         assert n in _lib.SYMBOLS, f"{n} has no ctypes prototype"
     assert set(_lib.SYMBOLS) == set(names)
-    assert _lib.lib().nlam_abi_version() == 2
+    assert _lib.lib().nlam_abi_version() == 3
     assert b"sm_90a" in _lib.lib().nlam_build_info()
 
 

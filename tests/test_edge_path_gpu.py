@@ -92,7 +92,7 @@ def _graph(case):
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_edge_path_selection(case):
+def test_edge_path_selection_and_support_queries(case):
     name, _, B, same, shared, upd, inplace_call, label, want_inplace, want_chain, want_encode = case
     L = _lib.lib()
     g = _graph(case)
@@ -125,8 +125,8 @@ def test_edge_path_selection(case):
     grid_rep = torch.empty(B, g.n_send, H, device=DEV)
     proj = torch.empty((B * g.n_send + g.n_rec) * H, device=DEV)
     got_encode = L.nlam_encode_supported(g.handle, ctypes.byref(ops.mlp_struct(embed_mlp)), src, 1,
-                                         ctypes.byref(ops.mlp_struct(grid_mlp)), ctypes.byref(em), r.data_ptr(), rbs,
-                                         e.data_ptr(), ebs, grid_rep.data_ptr(), proj.data_ptr(), g.n_send, B, 0)
+                                         ctypes.byref(ops.mlp_struct(grid_mlp)), ctypes.byref(em), None, r.data_ptr(), rbs,
+                                         e.data_ptr(), ebs, grid_rep.data_ptr(), proj.data_ptr(), None, None, g.n_send, B, 0)
     assert got_encode == want_encode
 
     # the same call with an edge pointer one float past a 16-byte boundary

@@ -5,8 +5,8 @@
   last 64-row tile is partial) and B = 1, 5, 32.  Bound (DESIGN §2): max |err| vs fp64 <= max(3 x the reference's own TF32
   error, 4e-3).
 * shapes the kernel does not cover (latent_dim 32, H = 128, hidden_layers 2, math fp32) compose and meet the same bound;
-* ``nlam_encode_emb_fwd``: grid_emb equals ``grid_prev_embedder.apply_rows`` bit for bit, its other outputs equal
-  ``nlam_encode_fwd``'s;
+* ``nlam_encode_fwd`` storing grid_emb: grid_emb equals ``grid_prev_embedder.apply_rows`` bit for bit, its other outputs
+  equal those of the call without grid_emb;
 * every golden case (reference Graph-EFM, stored noise) within the bound, and the parameter gradients of the case that has
   them within 2e-2 max|g| + 1e-4;
 * with the same noise the eager ``forward``, ``forward_with_boundary`` and a CUDA-graph replay are bit-identical; replays
@@ -166,7 +166,7 @@ def _inputs(m, B, seed):
             torch.randn(B, G, f, device=DEV, generator=gen))
 
 
-def test_encode_emb_outputs(config2):
+def test_encode_grid_emb_outputs(config2):
     m = config2[0]
     B = 3
     prev, prev_prev, forcing = _inputs(m, B, 1)
@@ -176,21 +176,22 @@ def test_encode_emb_outputs(config2):
     g = net._graph(prev.device)
     with torch.no_grad():
         with ops.profile_launches() as prof:
-            grid_rep, proj, grid_emb = ops.encode(g, m.grid_prev_embedder, sources, m.decoder.grid_update_mlp, net.edge_mlp,
-                                                  ge["mesh"], ge["g2m"], flags=net._flags(), want_emb=True)
+            grid_rep, (proj,), grid_emb = ops.encode(g, m.grid_prev_embedder, sources, m.decoder.grid_update_mlp, net.edge_mlp,
+                                                     ge["mesh"], ge["g2m"], flags=net._flags(), want_emb=True)
         assert prof.names() == ["tc_encode_kernel"], prof.names()
-        grid_rep0, proj0 = ops.encode(g, m.grid_prev_embedder, sources, m.decoder.grid_update_mlp, net.edge_mlp, ge["mesh"],
-                                      ge["g2m"], flags=net._flags())
+        grid_rep0, (proj0,), no_emb = ops.encode(g, m.grid_prev_embedder, sources, m.decoder.grid_update_mlp, net.edge_mlp,
+                                                 ge["mesh"], ge["g2m"], flags=net._flags())
         want_emb = m.grid_prev_embedder.apply_rows(sources)
+    assert no_emb is None
     assert torch.equal(grid_emb, want_emb), (grid_emb - want_emb).abs().max().item()
     assert torch.equal(grid_rep, grid_rep0) and torch.equal(proj, proj0)
 
 
-def test_encode_emb_abi_checks(config2):
+def test_encode_grid_emb_abi_checks(config2):
     m = config2[0]
     em = ops.mlp_struct(m.grid_prev_embedder)
-    rc = _lib.lib().nlam_encode_emb_fwd(None, ctypes.byref(em), None, 0, ctypes.byref(em), ctypes.byref(em), None, 0, None, 0,
-                                        None, None, None, 1, 1, 0, None)
+    rc = _lib.lib().nlam_encode_fwd(None, ctypes.byref(em), None, 0, ctypes.byref(em), ctypes.byref(em), None, None, 0, None, 0,
+                                    None, None, None, None, 1, 1, 0, None)
     assert rc == 1  # NLAM_E_INVALID
 
 

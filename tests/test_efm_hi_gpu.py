@@ -5,10 +5,11 @@
   path; case (a)'s parameter gradients within 2e-2 max|g| + 1e-4 of the reference's;
 * the launch list of the fused step (at the real size): ``tc_encode2_kernel`` first, one ``tc_latent_kernel``,
   ``tc_decode_kernel``, and no projection launch over grid rows besides the decoder's m2g projections;
-* ``nlam_encode2_fwd`` (tc_encode2_kernel): grid_rep and the first layer's projections equal ``nlam_encode_fwd``'s, the
-  second layer's equal the projections its own g2m call computes (tc_rowlinear_kernel) on the stored grid embedding, bit
-  for bit, and both layers' outputs equal their plain forward; a null argument returns NLAM_E_INVALID; its outputs are
-  closer to TF32 operands rounded to nearest than to truncated ones;
+* ``nlam_encode_fwd`` with a second g2m edge MLP (tc_encode2_kernel): grid_rep and the first layer's projections equal
+  those of the one-layer call, the second layer's equal the projections its own g2m call computes (tc_rowlinear_kernel) on
+  the stored grid embedding, bit for bit, and both layers' outputs equal their plain forward; a null argument, or a second
+  edge MLP together with grid_emb, returns NLAM_E_INVALID; its outputs are closer to TF32 operands rounded to nearest than
+  to truncated ones;
 * the stacked path that keeps its edge output (``GNNSequential(keep_stacked=True)``) equals the per-layer ``forward``;
 * with the same noise the eager ``forward``, ``forward_with_boundary`` and a CUDA-graph replay are bit-identical; replays
   after the same ``torch.cuda.manual_seed`` are bit-identical, members started from one state differ;
@@ -171,46 +172,63 @@ def _call_projections(net, send, mesh, edge):
 
 
 @pytest.mark.parametrize("B", [1, 3])
-def test_encode2_equals_the_launches_it_replaces(B):
+def test_encode_two_g2m_equals_the_launches_it_replaces(B):
     (emb, gm, a, b), sources, mesh, edge = _g2m_pair(B=B)
     G, N = sources[0].shape[1], mesh.shape[1]
     g = a._graph(mesh.device)
     with torch.no_grad():
         with ops.profile_launches() as prof:
-            grid_rep, proj, proj_b = ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=a._flags(),
-                                                edge_seq_b=b.edge_mlp)
+            grid_rep, (proj, proj_b), no_emb = ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=a._flags(),
+                                                          edge_seq_b=b.edge_mlp)
         assert prof.names() == ["tc_encode2_kernel"], prof.names()
-        grid_rep0, proj0, grid_emb = ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=a._flags(), want_emb=True)
+        grid_rep0, (proj0,), grid_emb = ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=a._flags(),
+                                                   want_emb=True)
         ps_b, pr_b, out_b = _call_projections(b, grid_emb, mesh, edge)
         _, _, out_a = _call_projections(a, grid_emb, mesh, edge)
         with ops.profile_launches() as prof:
-            rep_a, grid_rep2, rep_b = a.encode_step(emb, gm, sources, mesh, edge, second=b)
+            grid_rep2, (rep_a, rep_b), no_emb2 = a.encode_step(emb, gm, sources, mesh, edge, second=b)
         assert prof.names() == ["tc_encode2_kernel", "tc_edge_bcast_kernel", "tc_rowmlp_kernel", "tc_edge_bcast_kernel",
                                 "tc_rowmlp_kernel"], prof.names()
+    assert no_emb is None and no_emb2 is None
     assert torch.equal(grid_rep, grid_rep0) and torch.equal(proj, proj0)
     assert torch.equal(proj_b[:B * G * 64].view(B, G, 64), ps_b), (proj_b[:B * G * 64].view(B, G, 64) - ps_b).abs().max()
     assert torch.equal(proj_b[B * G * 64:].view(N, 64), pr_b), (proj_b[B * G * 64:].view(N, 64) - pr_b).abs().max()
     assert torch.equal(grid_rep2, grid_rep) and torch.equal(rep_a, out_a) and torch.equal(rep_b, out_b)
 
 
-def test_encode2_abi_checks():
+def test_encode_two_g2m_abi_checks():
     (emb, gm, a, b), sources, mesh, edge = _g2m_pair(B=1)
+    L = _lib.lib()
     em = ops.mlp_struct(emb)
-    rc = _lib.lib().nlam_encode2_fwd(None, ctypes.byref(em), None, 0, ctypes.byref(em), ctypes.byref(em), ctypes.byref(em),
-                                     None, 0, None, 0, None, None, None, 1, 1, 0, None)
+    rc = L.nlam_encode_fwd(None, ctypes.byref(em), None, 0, ctypes.byref(em), ctypes.byref(em), ctypes.byref(em), None, 0, None,
+                           0, None, None, None, None, 1, 1, 0, None)
     assert rc == 1  # NLAM_E_INVALID
     g = a._graph(mesh.device)
+    # grid_emb is not stored with a second edge MLP: the pair is not supported, and the call is invalid
+    G, N = sources[0].shape[1], mesh.shape[1]
+    grid_rep, grid_emb = torch.empty(1, G, 64, device=DEV), torch.empty(1, G, 64, device=DEV)
+    proj, proj_b = torch.empty((G + N) * 64, device=DEV), torch.empty((G + N) * 64, device=DEV)
+    gs, sa, sb = ops.mlp_struct(gm), ops.mlp_struct(a.edge_mlp), ops.mlp_struct(b.edge_mlp)
+    args = [g.handle, ctypes.byref(em), ops._row_srcs([ops.as_rows(t) for t in sources]), len(sources), ctypes.byref(gs),
+            ctypes.byref(sa), ctypes.byref(sb), mesh[0].data_ptr(), 0, edge[0].data_ptr(), 0, grid_rep.data_ptr(),
+            proj.data_ptr(), proj_b.data_ptr(), None, G, 1, 0]
+    assert L.nlam_encode_supported(*args) == 1
+    args[14] = grid_emb.data_ptr()
+    assert L.nlam_encode_supported(*args) == 0
+    assert L.nlam_encode_fwd(*args, None) == 1  # NLAM_E_INVALID
     # a second layer whose call does not take the batch-broadcast path (fp32 math) is declined, not approximated
     assert ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=_lib.MATH_FP32, edge_seq_b=b.edge_mlp) is None
 
 
-def test_encode2_rounds_operands_to_nearest():
+def test_encode_two_g2m_rounds_operands_to_nearest():
     """As test_tf32_rounding_gpu.py part B: tailed operands, fp64 references with operands rounded to nearest and truncated."""
     (emb, gm, a, b), sources, mesh, edge = _g2m_pair(G=1500, N=150, E=1400, B=2, tailed=True)
     g = a._graph(mesh.device)
     with torch.no_grad(), ops.profile_launches() as prof:
-        got = ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=_lib.MATH_TF32, edge_seq_b=b.edge_mlp)
+        grid_rep, projs, _ = ops.encode(g, emb, sources, gm, a.edge_mlp, mesh, edge, flags=_lib.MATH_TF32,
+                                        edge_seq_b=b.edge_mlp)
     assert prof.names() == ["tc_encode2_kernel"], prof.names()
+    got = [grid_rep, *projs]
     p64 = {f"{n}.{k}": v.detach().double() for n, m in (("e", emb), ("g", gm), ("a", a), ("b", b))
            for k, v in m.state_dict().items()}
     x64 = torch.cat([t.double() for t in sources], dim=-1)

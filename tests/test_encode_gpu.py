@@ -92,11 +92,13 @@ def _fused(m, sources):
         enc = ops.encode(g, m.grid_embedder, sources, m.encoding_grid_mlp, net.edge_mlp, mesh, g2m, flags=net._flags())
     assert enc is not None, "ops.encode does not cover this shape"
     assert prof.names() == ["tc_encode_kernel"], prof.names()
-    grid_rep, proj = enc
+    grid_rep, (proj,), grid_emb = enc
+    assert grid_emb is None
     ps, pr = proj[:B * G * 64].view(B, G, 64), proj[B * G * 64:].view(g.n_rec, 64)
     with ops.profile_launches() as prof:
-        mesh_rep, grid_rep2 = net.encode_step(m.grid_embedder, m.encoding_grid_mlp, sources, mesh, g2m)
+        grid_rep2, (mesh_rep,), grid_emb = net.encode_step(m.grid_embedder, m.encoding_grid_mlp, sources, mesh, g2m)
     assert prof.names() == ["tc_encode_kernel", "tc_edge_bcast_kernel", "tc_rowmlp_kernel"], prof.names()
+    assert grid_emb is None
     assert torch.equal(grid_rep2, grid_rep)
     return ps, pr, mesh_rep, grid_rep
 
@@ -111,7 +113,7 @@ def _check_equal(m, sources):
 
 
 @pytest.mark.parametrize("B", [1, 5, 32])
-def test_encode_config2_equals_three_launches(config2, B):
+def test_fused_encode_config2_equals_three_launches(config2, B):
     m, _ = config2
     assert m.num_grid_nodes % 64 != 0 and m.num_grid_nodes % 4 == 0
     _check_equal(m, _inputs(m, B, seed=B))
@@ -119,7 +121,7 @@ def test_encode_config2_equals_three_launches(config2, B):
 
 @pytest.mark.parametrize("B", [1, 2, 5])
 @pytest.mark.parametrize("dense_static", [False, True])
-def test_encode_misaligned_spans_and_partial_tile(B, dense_static):
+def test_fused_encode_misaligned_spans_and_partial_tile(B, dense_static):
     m, _ = _model(31, 26, P=1)
     assert m.num_grid_nodes % 4 == 2 and m.num_grid_nodes % 64 != 0
     _check_equal(m, _inputs(m, B, seed=10 + B, dense_static=dense_static))
@@ -176,11 +178,11 @@ def _supported(m, sources, grid_mlp_struct):
     proj = torch.empty((B * m.num_grid_nodes + g.n_rec) * 64, device=DEV)
     em, sm = ops.mlp_struct(m.grid_embedder), ops.mlp_struct(net.edge_mlp)
     return _lib.lib().nlam_encode_supported(g.handle, ctypes.byref(em), arr, len(sources), ctypes.byref(grid_mlp_struct),
-                                            ctypes.byref(sm), st["mesh_emb"].data_ptr(), 0, st["g2m_emb"].data_ptr(), 0,
-                                            out.data_ptr(), proj.data_ptr(), m.num_grid_nodes, B, net._flags())
+                                            ctypes.byref(sm), None, st["mesh_emb"].data_ptr(), 0, st["g2m_emb"].data_ptr(), 0,
+                                            out.data_ptr(), proj.data_ptr(), None, None, m.num_grid_nodes, B, net._flags())
 
 
-def test_encode_not_covered_without_layernorm_beta():
+def test_encode_query_declines_layernorm_without_beta():
     """The kernel reads every bias and LayerNorm parameter: an MLP whose LayerNorm has no shift is not covered."""
     m, _ = _model(31, 26, P=1)
     sources = _inputs(m, 2, seed=4)
