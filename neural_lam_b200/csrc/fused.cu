@@ -14,7 +14,10 @@
 // Launch names (nlam_profile_*): tc_rowmlp_kernel (row MLPs, node updates, output_map + step epilogue),
 // tc_rowlinear_kernel (node projections P_s = x_s·W1sᵀ, P_r = x_r·W1rᵀ + b1 of the split first edge Linear, both node
 // sets in one grid), tc_edge_kernel (K = 192 edge MLP on raw gathered rows), tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
-// epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).  The split-form edge stage
+// epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).  The node updates
+// (tc_node_proj_kernel, tc_node_out_kernel and the node-update form of tc_rowmlp_kernel) run on tc_node_kernel below, which
+// does this kernel's arithmetic with the next rows staged while the current ones compute; fused_mlp_kernel keeps them as the
+// fallback (node_pipelined).  The split-form edge stage
 // (first edge Linear split into e·W1eᵀ and node projections gathered in its epilogue) runs in tc_edge_split_kernel below
 // (tc_edge_split).  tc_edge_path decides, in one place, whether an edge stage takes the split or the K = 192 form and under
 // which label the split kernel is launched: tc_edge3_kernel (out-of-place edge output), tc_edge_rmw_kernel (edge tensor
@@ -1236,6 +1239,168 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_latent_kernel(const __grid_
   }
 }
 
+// ------------------------------------------------------------------------------------ H = 64 node update
+// The node update of an InteractionNet layer, out = res + LN(SiLU([src_0 | src_1]·Wn1ᵀ + bn1)·Wn2ᵀ + bn2) with res one of the
+// two 64-wide sources (rec for InteractionNet, aggr for PropagationNet), followed by one of fused_mlp_kernel's epilogues:
+//   POST_NONE    out                                                  (tc_rowmlp_kernel)
+//   POST_PROJ    out, P_s = out·W3ᵀ, P_r = out·W4ᵀ + b4               (tc_node_proj_kernel)
+//   POST_OUTMLP  step epilogue of SiLU(out·W3ᵀ + b3)·W4ᵀ + b4, out on chip   (tc_node_out_kernel)
+// The arithmetic is fused_mlp_kernel's, row for row: the same m64n64k8 MMAs in the same K order, the same TF32 rounding
+// points (operands rounded to nearest as they enter shared memory) and the same epilogue code, so the two kernels agree bit
+// for bit.  What differs is the load schedule.  Work items, warp-group ownership and staging are those of tc_latent_kernel:
+// an item is 64 rows of one batch element and belongs to one warp group; the item's two source spans (64 x 256 B each,
+// contiguous and 16-byte aligned) are copied with cp.async into the warp group's raw staging rows while the previous item's
+// GEMMs run.  cp.async does not round, so staging -> operand applies tf32r4 as fz_load_a does; the residual is read from
+// staging in fp32 into the accumulator fragment layout before the next item's copies overwrite it.
+namespace nod {
+using fz::CH_A;
+using fz::CH_W;
+constexpr int PITCH = 72;  // staged rows: 64 floats + 8 (fragment-layout float2 reads of a half warp hit distinct banks)
+constexpr uint32_t WN1 = 0, WN2 = WN1 + 4 * CH_W, W3 = WN2 + 2 * CH_W, W4 = W3 + 2 * CH_W;
+constexpr uint32_t A = W4 + 2 * CH_W;                  // 128 x 128 operand [src_0 | src_1], 64 rows per warp group
+constexpr uint32_t STG = A + 4 * CH_A;                 // per warp group: 64 src_0 rows | 64 src_1 rows, PITCH floats each
+constexpr uint32_t STG_WG = 2 * 64 * PITCH * 4;
+constexpr uint32_t PRM = STG + 2 * STG_WG;             // bn1 | bn2 | gamma | beta | b3 | b4
+constexpr uint32_t BYTES = PRM + 6 * 64 * 4 + 1024;    // + alignment slack
+static_assert(BYTES <= 227 * 1024, "node kernel shared memory exceeds the sm_90 limit");
+}  // namespace nod
+
+struct NodeParams {
+  int B, post, res_src;       // post: fz::Post; res_src: the source that is also the residual
+  long long n_rows, n_tiles;  // rows; 64-row tiles per batch element
+  const float* src[2];        // (B | 1, n_rows, 64), batch stride bs (0: shared by the batch)
+  long long bs[2];
+  FzW wn1, wn2, w3, w4;
+  const float *bn1, *bn2, *gamma, *beta, *b3, *b4;
+  float eps;
+  float* out;                 // (B, n_rows, out_w)
+  int out_w;
+  float *out3, *out4;         // POST_PROJ: (B, n_rows, 64) each
+  const float *prev, *bnd, *mask, *dstd, *dmean;  // POST_OUTMLP: the forecast-step epilogue
+};
+
+__global__ void __launch_bounds__(fz::THREADS, 1) tc_node_kernel(const __grid_constant__ NodeParams p) {
+  using namespace fz;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const uint32_t sb = smem_u32(s);
+  uint8_t* sA = s + nod::A;
+  float* prm = reinterpret_cast<float*>(s + nod::PRM);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
+  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // operand row of fragment half 0 (half 1: + 8)
+  const int lr = rq - 64 * wg;                              // the same row within the warp group's 64
+  const int cq = 2 * (lane & 3);
+  const uint32_t aA = sb + nod::A + wg * (CH_A / 2);
+  const float* stg = reinterpret_cast<const float*>(s + nod::STG + wg * nod::STG_WG);
+  const float* sres = stg + p.res_src * 64 * nod::PITCH;
+  const uint32_t stg_u = smem_u32(stg);
+
+  fz_load_w(s + nod::WN1, p.wn1, 4, tid);
+  fz_load_w(s + nod::WN2, p.wn2, 2, tid);
+  if (p.post != POST_NONE) {
+    fz_load_w(s + nod::W3, p.w3, 2, tid);
+    fz_load_w(s + nod::W4, p.w4, 2, tid);
+  }
+  for (int i = tid; i < 64; i += THREADS) {  // the defaults of fused_mlp_kernel
+    prm[i] = p.bn1 ? p.bn1[i] : 0.f;
+    prm[64 + i] = p.bn2 ? p.bn2[i] : 0.f;
+    prm[128 + i] = p.gamma[i];
+    prm[192 + i] = p.beta ? p.beta[i] : 0.f;
+    prm[256 + i] = p.b3 ? p.b3[i] : 0.f;
+    prm[320 + i] = p.b4 ? p.b4[i] : 0.f;
+  }
+  fence_proxy_async();
+  __syncthreads();  // the last CTA-wide barrier: from here on each warp group runs on its own
+
+  const long long n_items = p.n_tiles * p.B, stride = 2LL * gridDim.x;
+  const uint64_t pol_stream = policy_evict_first(), pol_shared = policy_evict_normal();
+  // the rows of item it -> staging: source q's 64 rows at float 64 PITCH q, one 16-byte aligned span per source
+  auto issue = [&](long long it) {
+    const int bi = (int)(it / p.n_tiles);
+    const long long row0 = (it - (long long)bi * p.n_tiles) * 64;
+    const int n = (int)min(64LL, p.n_rows - row0);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const float* g = p.src[q] + bi * p.bs[q] + row0 * 64;
+      const uint32_t dst = stg_u + 4u * (uint32_t)(q * 64 * nod::PITCH);
+      const uint64_t pol = p.bs[q] ? pol_stream : pol_shared;
+      for (int k = gt; k < n * 16; k += 128) cp_async_16(dst + 4u * (uint32_t)((k >> 4) * nod::PITCH + (k & 15) * 4), g + 4 * k, pol);
+    }
+  };
+  float acc[32];
+  float v[2][16], r[2][16];
+  long long item = 2LL * blockIdx.x + wg;
+  if (item < n_items) issue(item);
+  for (; item < n_items; item += stride) {
+    const int b = (int)(item / p.n_tiles);
+    const long long row0 = (item - (long long)b * p.n_tiles) * 64;
+    const int nrows = (int)min(64LL, p.n_rows - row0);
+    const bool valid0 = lr < nrows, valid1 = lr + 8 < nrows;
+    // ---- 1. staged rows -> operand (TF32, zero rows past the end); this thread's residual in the fragment layout (fp32)
+    cp_async_wait_all();
+    named_bar_sync(bar, 128);  // every thread's copies have landed; the previous item's MMAs are done with the operand
+    for (int g = gt; g < 64 * 32; g += 128) {
+      const int i = g >> 5, c = (g & 31) * 4;
+      const float4 x = i < nrows ? *reinterpret_cast<const float4*>(stg + (c >> 6) * 64 * nod::PITCH + i * nod::PITCH + (c & 63))
+                                 : make_float4(0.f, 0.f, 0.f, 0.f);
+      *reinterpret_cast<float4*>(sA + fz_off(CH_A, 64 * wg + i, c)) = tf32r4(x);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 x = (i ? valid1 : valid0) ? *reinterpret_cast<const float2*>(sres + (lr + 8 * i) * nod::PITCH + 8 * j + cq)
+                                               : make_float2(0.f, 0.f);
+        r[i][2 * j] = x.x;
+        r[i][2 * j + 1] = x.y;
+      }
+    fence_proxy_async();
+    named_bar_sync(bar, 128);  // the operand is complete and the staging rows free
+    if (item + stride < n_items) issue(item + stride);
+    // ---- 2. node MLP on [src_0 | src_1], LayerNorm, residual
+    fz_gemm(acc, aA, sb + nod::WN1, 4);
+    fz_unpack(acc, v, prm);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+    fz_store_op(sA, v, rq, wg);
+    fz_gemm(acc, aA, sb + nod::WN2, 2);
+    fz_unpack(acc, v, prm + 64);
+    fz_layernorm(v, prm + 128, prm + 192, p.eps);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] += r[i][t];
+    const long long r0 = row0 + lr;
+    // ---- 3. epilogue
+    if (p.post == POST_NONE) {
+      fz_store_rows(p, p.out, 64, p.n_rows, false, v, b, r0, valid0, valid1);
+    } else if (p.post == POST_PROJ) {
+      fz_store_rows(p, p.out, 64, p.n_rows, false, v, b, r0, valid0, valid1);  // the updated node rows
+      fz_store_op(sA, v, rq, wg);
+      fz_gemm(acc, aA, sb + nod::W3, 2);
+      fz_unpack(acc, v, nullptr);
+      fz_store_rows(p, p.out3, 64, p.n_rows, false, v, b, r0, valid0, valid1);
+      fz_gemm(acc, aA, sb + nod::W4, 2);
+      fz_unpack(acc, v, prm + 320);
+      fz_store_rows(p, p.out4, 64, p.n_rows, false, v, b, r0, valid0, valid1);
+    } else {  // POST_OUTMLP: the updated node rows stay on chip
+      fz_store_op(sA, v, rq, wg);
+      fz_gemm(acc, aA, sb + nod::W3, 2);
+      fz_unpack(acc, v, prm + 256);
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
+      fz_store_op(sA, v, rq, wg);
+      fz_gemm(acc, aA, sb + nod::W4, 2);
+      fz_unpack(acc, v, prm + 320);
+      fz_store_rows(p, p.out, p.out_w, p.n_rows, true, v, b, r0, valid0, valid1);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------ host
 static FzW wslice(const float* w, int ld, int rows, int cols) { return FzW{w, ld, rows, cols}; }
 
@@ -1258,6 +1423,70 @@ static int fz_launch(const FzParams& p, const char* name, double bytes, cudaStre
   {
     ProfScope ps(name, st, bytes);
     fused_mlp_kernel<<<grid, fz::THREADS, smem, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
+}
+
+// Whether the node update p (fz_node's two 64-wide sources, a residual equal to one of them, LayerNorm, out_w 64 or a step
+// epilogue) runs on tc_node_kernel: both sources 16-byte aligned with batch strides % 4 == 0 (one aligned cp.async span per
+// item), unless NLAM_TC_NODE=v1 asks for fused_mlp_kernel.  Read at every call, so that one process can run both kernels on
+// the same inputs; the two agree bit for bit.
+static bool node_pipelined(const FzParams& p) {
+  const char* e = getenv("NLAM_TC_NODE");
+  if (e && e[0] == 'v' && e[1] == '1') return false;
+  for (int q = 0; q < 2; ++q)
+    if (!aligned16(p.src[q].ptr) || p.src[q].bs % 4 != 0) return false;
+  return true;
+}
+
+static int node_launch(const FzParams& f, int res_src, const char* name, double bytes, cudaStream_t st) {
+  NodeParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = f.B;
+  p.post = f.post;
+  p.res_src = res_src;
+  p.n_rows = f.n_rows;
+  p.n_tiles = (f.n_rows + 63) / 64;
+  for (int q = 0; q < 2; ++q) {
+    p.src[q] = f.src[q].ptr;
+    p.bs[q] = f.src[q].bs;
+  }
+  p.wn1 = f.w1;
+  p.wn2 = f.w2;
+  p.w3 = f.w3;
+  p.w4 = f.w4;
+  p.bn1 = f.b1;
+  p.bn2 = f.b2;
+  p.gamma = f.gamma;
+  p.beta = f.beta;
+  p.b3 = f.b3;
+  p.b4 = f.b4;
+  p.eps = f.eps;
+  p.out = f.out;
+  p.out_w = f.out_w;
+  p.out3 = f.out3;
+  p.out4 = f.out4;
+  p.prev = f.prev;
+  p.bnd = f.bnd;
+  p.mask = f.mask;
+  p.dstd = f.dstd;
+  p.dmean = f.dmean;
+  const long long n_items = p.n_tiles * p.B;
+  if (n_items == 0) return NLAM_OK;
+  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  static unsigned mask = 0;
+  if (!(mask & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_node_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nod::BYTES));
+    mask |= 1u << (dev & 31);
+  }
+  const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
+  {
+    ProfScope ps(name, st, bytes);
+    tc_node_kernel<<<grid, fz::THREADS, nod::BYTES, st>>>(p);
   }
   count_launch();
   NLAM_CUDA_OK(cudaGetLastError());
@@ -1297,6 +1526,12 @@ static void fz_mlp(FzParams& p, const NlamMlp* m, int k_off, int k_cols) {
   p.gamma = m->ln_gamma;
   p.beta = m->ln_beta;
   p.eps = m->ln_eps;
+}
+
+// node MLP: [rec | aggr] (128) -> 64 -> 64 with an affine LayerNorm
+static bool node_mlp_ok(const NlamMlp* m) {
+  int no = 0;
+  return mlp_shape_ok(m, &no) && no == 64 && m->in_dim == 128 && m->ln_gamma && m->ln_beta;
 }
 
 // ---- row MLPs (H = 64): embedders, node updates, output_map (+ step epilogue)
@@ -1363,6 +1598,11 @@ int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamR
     p.dmean = ep->mean;
     bytes += 4.0 * n_rows * B * nout * (ep->boundary ? 2 : 1);
   }
+  // node update: two 64-wide sources, the residual one of them
+  int res_src = -1;
+  if (res && !ep && n_src == 2 && srcs[0].dim == 64 && srcs[1].dim == 64 && node_mlp_ok(mlp))
+    res_src = (srcs[0].ptr == res->ptr && srcs[0].bstride == res->bstride) ? 0 : 1;
+  if (res_src >= 0 && node_pipelined(p)) return node_launch(p, res_src, "tc_rowmlp_kernel", bytes, st);
   return fz_launch(p, "tc_rowmlp_kernel", bytes, st);
 }
 
@@ -1535,10 +1775,6 @@ int tc_edge(const NlamGraph* g, const NlamMlp* edge_mlp, const float* send, int6
 }
 
 // ---- node update chained with the next layer's projections / with output_map + step epilogue
-static bool node_mlp_ok(const NlamMlp* m) {
-  int no = 0;
-  return mlp_shape_ok(m, &no) && no == 64 && m->in_dim == 128 && m->ln_gamma && m->ln_beta;
-}
 
 bool tc_node_proj_supported(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs,
                             const float* aggr, int64_t n_rows, const float* out, const float* proj_out) {
@@ -1577,7 +1813,9 @@ int tc_node_proj(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const fl
   p.b4 = next_edge_mlp->b[0];
   p.out3 = proj_out;
   p.out4 = proj_out + (size_t)B * n_rows * 64;
-  return fz_launch(p, "tc_node_proj_kernel", 4.0 * n_rows * 64 * (((rec_bs != 0 && B > 1) ? B : 1) + 4.0 * B), st);
+  const double bytes = 4.0 * n_rows * 64 * (((rec_bs != 0 && B > 1) ? B : 1) + 4.0 * B);
+  if (node_pipelined(p)) return node_launch(p, 0, "tc_node_proj_kernel", bytes, st);
+  return fz_launch(p, "tc_node_proj_kernel", bytes, st);
 }
 
 bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
@@ -1611,7 +1849,9 @@ int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* re
   p.mask = ep->mask;
   p.dstd = ep->std;
   p.dmean = ep->mean;
-  return fz_launch(p, "tc_node_out_kernel", 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + 3.0 * D * B), st);
+  const double bytes = 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + 3.0 * D * B);
+  if (node_pipelined(p)) return node_launch(p, 0, "tc_node_out_kernel", bytes, st);
+  return fz_launch(p, "tc_node_out_kernel", bytes, st);
 }
 
 // ---- mesh -> grid decoder: edge projections (tc_rowlinear_kernel) + tc_decode_kernel
