@@ -661,18 +661,32 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_edge_split_kernel(const __g
 //   aggr  = sum (or mean) of the m_k                          (warp shuffles, on chip)
 //   grid' = rec + LN(SiLU([rec | aggr]·Wn1ᵀ + bn1)·Wn2ᵀ + bn2)
 //   new   = step epilogue of SiLU(grid'·Wo1ᵀ + bo1)·Wo2ᵀ + bo2
-// A work item is 64 receivers of one batch element and belongs to one warp group; the two warp groups of a CTA share only
-// the weights and synchronise on their own named barriers, so one group's loads overlap the other's MMAs.  Items run
-// batch-fastest: the B items of one receiver block run at about the same time and read its P_e rows from L2.
+// A work item is 64 receivers of one batch element.  The CTA is warp-specialized: warp group 0 loads, warp groups 1 and 2
+// compute, one item at a time each; items run batch-fastest, so the B items of one receiver block run at about the same
+// time and read its P_e rows from L2.  Half of the load warp group (64 threads) feeds each compute warp group through a
+// ring of RING units in shared memory, 64 rows x 64 fp32 each in the operands' 128-byte swizzle, signalled by full / empty
+// mbarriers.  Per item the stream is the receiver rows, then for each sub-tile of 64 edges the sums P_e[k] + P_s[b, src[k]]
+// (added by the load warps in the order the edge pre-activation adds them).  The load warps hold a whole unit in flight in
+// registers and fetch the next sub-tile's sender indices behind it, and they prefetch the item's previous / boundary state
+// rows into L2 for the epilogue.  The compute warps read the receiver rows from the ring in fp32 into the accumulator
+// layout (the residual, kept in registers) and round them in place to TF32 for P_r and the first half of node GEMM 1
+// (K = 64 of 128, its accumulators kept in registers), which frees the unit one item ahead; each sub-tile's SiLU(...) is
+// written (TF32) over the sums it was computed from and is the edge GEMM's operand.  Every operand is rounded to nearest
+// before an MMA reads it, and every sum, K order and rounding point is that of the node-update and edge paths.
 namespace dec {
 using fz::CH_A;
 using fz::CH_W;
+constexpr int THREADS = 384;  // warp group 0 loads, warp groups 1 and 2 compute
+constexpr int RING = 2;       // ring units per compute warp group
 constexpr uint32_t W1R = 0, W2E = W1R + 2 * CH_W, WN1 = W2E + 2 * CH_W, WN2 = WN1 + 4 * CH_W, WO1 = WN2 + 2 * CH_W,
                    WO2 = WO1 + 2 * CH_W;
-constexpr uint32_t NODE = WO2 + 2 * CH_W;  // 128 x 128 operand: [rec | P_r, then aggr]
-constexpr uint32_t EDGE = NODE + 4 * CH_A;  // 128 x 64 operand: hidden edge activations
-constexpr uint32_t PRM = EDGE + 2 * CH_A;   // b2, gamma, beta (edge MLP) | bn1, bn2, gamma, beta (node MLP) | bo1, bo2
-constexpr uint32_t BYTES = PRM + 9 * 64 * 4 + 1024;  // + alignment slack
+constexpr uint32_t NODE = WO2 + 2 * CH_W;  // 128 x 64 operand, 64 rows per compute warp group: P_r (fp32), then aggr, then
+                                           // the node / output GEMMs' operands
+constexpr uint32_t SLOT = 2 * CH_A;        // one ring slot: 128 x 64, the unit of compute warp group c in rows 64c ..
+constexpr uint32_t RINGS = NODE + 2 * CH_A;
+constexpr uint32_t PRM = RINGS + RING * SLOT;  // b2, gamma, beta (edge MLP) | bn1, bn2, gamma, beta (node MLP) | bo1, bo2
+constexpr uint32_t BAR = PRM + 9 * 64 * 4;     // full[c][slot] (64 arrivals: the load threads), empty[c][slot] (128)
+constexpr uint32_t BYTES = BAR + 2 * 2 * RING * 8 + 1024;  // + alignment slack
 static_assert(BYTES <= 227 * 1024, "decoder shared memory exceeds the sm_90 limit");
 }  // namespace dec
 
@@ -692,28 +706,38 @@ struct DecParams {
   const float *prev, *bnd, *mask, *dstd, *dmean;
 };
 
+// warp group MMA that adds to the accumulators: acc += A[rows] · Wᵀ over kc chunks
+__device__ __forceinline__ void dec_gemm_add(float* acc, uint32_t a, uint32_t w, int kc) {
+  wgmma_fence(acc, 32);
+  for (int c = 0; c < kc; ++c) {
+    const uint64_t da = gmma_desc(a + c * fz::CH_A), db = gmma_desc(w + c * fz::CH_W);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) Wgmma<64>::mma(acc, da + 2 * k, db + 2 * k, 1u);
+  }
+  wgmma_commit();
+  wgmma_wait0(acc, 32);
+}
+
 template <int DEG>  // uniform in-degree: 1, 2, 4 or 8
-__global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_constant__ DecParams p) {
+__global__ void __launch_bounds__(dec::THREADS, 1) tc_decode_kernel(const __grid_constant__ DecParams p) {
   using namespace fz;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const uint32_t sb = smem_u32(s);
-  uint8_t* sN = s + dec::NODE;
-  uint8_t* sE = s + dec::EDGE;
   float* prm = reinterpret_cast<float*>(s + dec::PRM);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, gt = tid & 127, bar = 1 + wg;
-  const int rq = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // operand row of fragment half 0 (half 1: + 8)
-  const int lr = rq - 64 * wg;                              // the same row within the warp group's 64
-  const int cq = 2 * (lane & 3);
-  const uint32_t aN = sb + dec::NODE + wg * (CH_A / 2), aE = sb + dec::EDGE + wg * (CH_A / 2);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2;
+  auto full = [&](int c, uint32_t slot) { return sb + dec::BAR + 8u * (uint32_t)(c * dec::RING + slot); };
+  auto empty = [&](int c, uint32_t slot) { return sb + dec::BAR + 8u * (uint32_t)((2 + c) * dec::RING + slot); };
 
-  fz_load_w(s + dec::W1R, p.w1r, 2, tid);
-  fz_load_w(s + dec::W2E, p.w2e, 2, tid);
-  fz_load_w(s + dec::WN1, p.wn1, 4, tid);
-  fz_load_w(s + dec::WN2, p.wn2, 2, tid);
-  fz_load_w(s + dec::WO1, p.wo1, 2, tid);
-  fz_load_w(s + dec::WO2, p.wo2, 2, tid);
-  for (int i = tid; i < 64; i += THREADS) {
+  if (tid < THREADS) {
+    fz_load_w(s + dec::W1R, p.w1r, 2, tid);
+    fz_load_w(s + dec::W2E, p.w2e, 2, tid);
+    fz_load_w(s + dec::WN1, p.wn1, 4, tid);
+    fz_load_w(s + dec::WN2, p.wn2, 2, tid);
+    fz_load_w(s + dec::WO1, p.wo1, 2, tid);
+    fz_load_w(s + dec::WO2, p.wo2, 2, tid);
+  }
+  for (int i = tid; i < 64; i += dec::THREADS) {
     prm[i] = p.b2e[i];
     prm[64 + i] = p.gamma_e[i];
     prm[128 + i] = p.beta_e[i];
@@ -724,87 +748,147 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_
     prm[448 + i] = p.bo1[i];
     prm[512 + i] = i < p.D ? p.bo2[i] : 0.f;
   }
+  if (tid == 0)
+    for (int c = 0; c < 2; ++c)
+      for (uint32_t k = 0; k < dec::RING; ++k) {
+        mbar_init(full(c, k), 64);
+        mbar_init(empty(c, k), 128);
+      }
   fence_proxy_async();
-  __syncthreads();  // the last CTA-wide barrier: from here on each warp group runs on its own
+  __syncthreads();  // the last CTA-wide barrier: from here on the load halves and compute warp groups run in pairs
 
-  const float scale = p.mean ? 1.f / (float)DEG : 1.f;
   const long long n_items = p.n_blocks * p.B;
   const long long stride = 2LL * gridDim.x;
-  // Loads run one stage ahead of their use: the next item's receiver rows and sender indices are issued before this
-  // item's node / output GEMMs, each sub-tile's P_e / P_s rows before the previous sub-tile's GEMM.
-  float4 x[8];         // receiver rows of the item: 64 rows x 16 float4 over the warp group's 128 threads
-  int sidx[DEG][2];    // sender of each edge row of the thread, per sub-tile
-  float2 pe[2][8], ps[2][8];
-  auto load_item = [&](long long it) {
-    const int bi = (int)(it % p.B);
-    const long long ri = (it / p.B) * 64;
-    const float* rec = p.rec + (long long)bi * p.rec_bs;
+  if (wg == 0) {
+    // ---- load warps: threads 64c .. 64c + 63 feed compute warp group c.  Thread pt moves float4 column q4 of the unit's
+    // rows pt / 16 + 4k, k < 16.
+    const int c = tid >> 6, pt = tid & 63, q4 = (pt & 15) * 4, row = pt >> 4;
+    uint32_t u = 0;  // units sent
+    float4 x[16], y[16];
+    int sidx[16];    // sender of each edge row of the thread in the coming sub-tile (-1: past the last receiver)
+    auto put = [&]() {
+      const uint32_t slot = u % dec::RING;
+      mbar_wait_nocall(empty(c, slot), ((u / dec::RING) & 1) ^ 1);
+      uint8_t* dst = s + dec::RINGS + slot * dec::SLOT;
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const long long r = ri + 8 * q + (gt >> 4);
-      x[q] = r < p.n_rec ? __ldg(reinterpret_cast<const float4*>(rec + r * 64 + (gt & 15) * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+      for (int k = 0; k < 16; ++k) *reinterpret_cast<float4*>(dst + fz_off(CH_A, 64 * c + row + 4 * k, q4)) = x[k];
+      mbar_arrive(full(c, slot));
+      ++u;
+    };
+    for (long long item = 2LL * blockIdx.x + c; item < n_items; item += stride) {
+      const int b = (int)(item % p.B);
+      const long long r0 = (item / p.B) * 64;
+      const float* rec = p.rec + (long long)b * p.rec_bs;
 #pragma unroll
-    for (int st = 0; st < DEG; ++st)
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int e = st * 64 + lr + 8 * i;  // edge within the item; its receiver is e / DEG
-        sidx[st][i] = ri + e / DEG < p.n_rec ? __ldg(p.src + ri * DEG + e) : -1;
+      for (int k = 0; k < 16; ++k) {
+        const long long r = r0 + row + 4 * k;
+        x[k] = r < p.n_rec ? __ldg(reinterpret_cast<const float4*>(rec + r * 64 + q4)) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
-  };
-  auto gather = [&](int st, int bi, long long ri) {
+      auto load_src = [&](int st) {
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const bool ok = sidx[st][i] >= 0;
-      const float* pk = p.pe + (ri * DEG + st * 64 + lr + 8 * i) * 64;
-      const float* sk = p.ps + (long long)bi * p.ps_bs + (long long)(ok ? sidx[st][i] : 0) * 64;
+        for (int k = 0; k < 16; ++k) {
+          const int e = st * 64 + row + 4 * k;  // edge within the item; its receiver is e / DEG
+          sidx[k] = r0 + e / DEG < p.n_rec ? __ldg(p.src + r0 * DEG + e) : -1;
+        }
+      };
+      load_src(0);
+      {  // the epilogue's previous / boundary state rows of the item -> L2
+        const long long n = min(64LL, p.n_rec - r0) * p.D;
+        const float* spans[2] = {p.prev + ((long long)b * p.n_rec + r0) * p.D, p.bnd ? p.bnd + ((long long)b * p.n_rec + r0) * p.D : nullptr};
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        pe[i][j] = ok ? __ldg(reinterpret_cast<const float2*>(pk + 8 * j + cq)) : make_float2(0.f, 0.f);
-        ps[i][j] = ok ? __ldg(reinterpret_cast<const float2*>(sk + 8 * j + cq)) : make_float2(0.f, 0.f);
+        for (int q = 0; q < 2; ++q) {
+          if (!spans[q]) continue;
+          const uintptr_t a0 = (uintptr_t)spans[q] & ~(uintptr_t)127, a1 = (uintptr_t)(spans[q] + n);
+          for (uintptr_t a = a0 + 128u * (uintptr_t)pt; a < a1; a += 128u * 64u) prefetch_l2(reinterpret_cast<const void*>(a));
+        }
+      }
+      put();
+#pragma unroll 1
+      for (int st = 0; st < DEG; ++st) {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+          const bool ok = sidx[k] >= 0;
+          const float* pk = p.pe + (r0 * DEG + st * 64 + row + 4 * k) * 64 + q4;
+          const float* sk = p.ps + (long long)b * p.ps_bs + (long long)(ok ? sidx[k] : 0) * 64 + q4;
+          x[k] = ok ? __ldg(reinterpret_cast<const float4*>(pk)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          y[k] = ok ? __ldg(reinterpret_cast<const float4*>(sk)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        if (st + 1 < DEG) load_src(st + 1);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) x[k] = make_float4(x[k].x + y[k].x, x[k].y + y[k].y, x[k].z + y[k].z, x[k].w + y[k].w);
+        put();
       }
     }
-  };
-  float acc[32];
-  float v[2][16];
-  long long item = 2LL * blockIdx.x + wg;
-  if (item < n_items) load_item(item);
-  for (; item < n_items; item += stride) {
+    return;
+  }
+
+  // ---- compute warps
+  const int c = wg - 1, bar = 1 + c;
+  const int lr = 16 * (warp & 3) + (lane >> 2);  // row of fragment half 0 within the warp group's 64 (half 1: + 8)
+  const int rq = 64 * c + lr;                     // the same row in a 128-row operand
+  const int cq = 2 * (lane & 3);
+  uint8_t* sN = s + dec::NODE;
+  const uint32_t aN = sb + dec::NODE + c * (CH_A / 2);
+  const float scale = p.mean ? 1.f / (float)DEG : 1.f;
+  float acc[32], acc1[32];  // acc1: node GEMM 1, from the receiver rows until the aggregate is added
+  float v[2][16], res[2][16];
+  uint32_t u = 0;  // units received
+  for (long long item = 2LL * blockIdx.x + c; item < n_items; item += stride) {
     const int b = (int)(item % p.B);
     const long long r0 = (item / p.B) * 64;
-    const float* rec = p.rec + (long long)b * p.rec_bs;
-    gather(0, b, r0);
-    // ---- 1. the item's 64 receiver rows -> node operand chunks 0-1 (TF32)
-    named_bar_sync(bar, 128);  // the previous item's MMAs have finished reading the node operand
+    // ---- 1. receiver rows: the residual in fp32, the operand rounded in place; P_r and node GEMM 1 on chunks 0-1
+    uint32_t slot = u % dec::RING;
+    uint8_t* sU = s + dec::RINGS + slot * dec::SLOT;
+    uint32_t aU = sb + dec::RINGS + slot * dec::SLOT + c * (CH_A / 2);
+    mbar_wait_nocall(full(c, slot), (u / dec::RING) & 1);
 #pragma unroll
-    for (int q = 0; q < 8; ++q)
-      *reinterpret_cast<float4*>(sN + fz_off(CH_A, 64 * wg + 8 * q + (gt >> 4), (gt & 15) * 4)) = tf32r4(x[q]);
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float2* px = reinterpret_cast<float2*>(sU + fz_off(CH_A, rq + 8 * i, 8 * j + cq));
+        const float2 x = *px;
+        res[i][2 * j] = x.x;
+        res[i][2 * j + 1] = x.y;
+        *px = make_float2(tf32r(x.x), tf32r(x.y));
+      }
     fence_proxy_async();
     named_bar_sync(bar, 128);
-    // ---- 2. P_r = rec·W1rᵀ, kept in fp32 in chunks 2-3 (an addend of the edge pre-activation, not an MMA operand)
-    fz_gemm(acc, aN, sb + dec::W1R, 2);
+    fz_gemm(acc, aU, sb + dec::W1R, 2);
+    fz_gemm(acc1, aU, sb + dec::WN1, 2);
+    mbar_arrive(empty(c, slot));
+    ++u;
+    // P_r, kept in fp32 (an addend of the edge pre-activation, not an MMA operand).  The previous item's last MMA read of
+    // the node operand ended before the barrier above.
     fz_unpack(acc, v, nullptr);
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
       for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float2*>(sN + fz_off(CH_A, rq + 8 * i, 64 + 8 * j + cq)) = make_float2(v[i][2 * j], v[i][2 * j + 1]);
+        *reinterpret_cast<float2*>(sN + fz_off(CH_A, rq + 8 * i, 8 * j + cq)) = make_float2(v[i][2 * j], v[i][2 * j + 1]);
     named_bar_sync(bar, 128);  // every P_r row of the item is visible to the whole warp group
-    // ---- 3. edges: DEG sub-tiles of 64 edges = 64 / DEG receivers each
-#pragma unroll
+    // ---- 2. edges: DEG sub-tiles of 64 edges = 64 / DEG receivers each
+#pragma unroll 1
     for (int st = 0; st < DEG; ++st) {
       const int rl0 = (st * 64 + lr) / DEG, rl1 = (st * 64 + lr + 8) / DEG;  // receivers of the two fragment rows
+      slot = u % dec::RING;
+      sU = s + dec::RINGS + slot * dec::SLOT;
+      aU = sb + dec::RINGS + slot * dec::SLOT + c * (CH_A / 2);
+      mbar_wait_nocall(full(c, slot), (u / dec::RING) & 1);
+      // SiLU(P_e + P_s + P_r) over the sums it is computed from: each thread rewrites exactly the elements it reads
 #pragma unroll
       for (int i = 0; i < 2; ++i)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const float2 pr = *reinterpret_cast<const float2*>(sN + fz_off(CH_A, 64 * wg + (i ? rl1 : rl0), 64 + 8 * j + cq));
-          v[i][2 * j] = silu_fast(pe[i][j].x + ps[i][j].x + pr.x);
-          v[i][2 * j + 1] = silu_fast(pe[i][j].y + ps[i][j].y + pr.y);
+          float2* pq = reinterpret_cast<float2*>(sU + fz_off(CH_A, rq + 8 * i, 8 * j + cq));
+          const float2 q = *pq;
+          const float2 pr = *reinterpret_cast<const float2*>(sN + fz_off(CH_A, 64 * c + (i ? rl1 : rl0), 8 * j + cq));
+          *pq = make_float2(tf32r(silu_fast(q.x + pr.x)), tf32r(silu_fast(q.y + pr.y)));
         }
-      if (st + 1 < DEG) gather(st + 1, b, r0);
-      fz_store_op(sE, v, rq, wg);  // its barriers also mean every P_r read of this sub-tile is done
-      fz_gemm(acc, aE, sb + dec::W2E, 2);
+      fence_proxy_async();
+      named_bar_sync(bar, 128);  // the edge operand is complete, and every P_r read of this sub-tile is done
+      fz_gemm(acc, aU, sb + dec::W2E, 2);
+      mbar_arrive(empty(c, slot));
+      ++u;
       fz_unpack(acc, v, prm);
       fz_layernorm(v, prm + 64, prm + 128, p.eps_e);
       // per-receiver sum: the DEG edges of a receiver are consecutive fragment rows, held by lanes 4, 8 and 16 apart
@@ -824,38 +908,40 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_decode_kernel(const __grid_
         for (int i = 0; i < 2; ++i)
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<float2*>(sN + fz_off(CH_A, 64 * wg + (i ? rl1 : rl0), 64 + 8 * j + cq)) =
+            *reinterpret_cast<float2*>(sN + fz_off(CH_A, 64 * c + (i ? rl1 : rl0), 8 * j + cq)) =
                 make_float2(tf32r(v[i][2 * j]), tf32r(v[i][2 * j + 1]));
       }
     }
-    if (item + stride < n_items) load_item(item + stride);
     fence_proxy_async();
     named_bar_sync(bar, 128);
-    // ---- 4. node MLP on [rec | aggr] + residual, output_map, step epilogue (as the POST_OUTMLP path of fused_mlp_kernel)
-    fz_gemm(acc, aN, sb + dec::WN1, 4);
-    fz_unpack(acc, v, prm + 192);
+    // ---- 3. node MLP on [rec | aggr] (chunks 2-3 of Wn1 on aggr) + residual, output_map, step epilogue (as the
+    // POST_OUTMLP path of tc_node_kernel)
+    dec_gemm_add(acc1, aN, sb + dec::WN1 + 2 * CH_W, 2);
+    fz_unpack(acc1, v, prm + 192);
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
       for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
-    fz_store_op(sN, v, rq, wg);
+    fz_store_op(sN, v, rq, c);
     fz_gemm(acc, aN, sb + dec::WN2, 2);
     fz_unpack(acc, v, prm + 256);
     fz_layernorm(v, prm + 320, prm + 384, p.eps_n);
-    const long long ra = r0 + lr;
-    const bool valid0 = ra < p.n_rec, valid1 = ra + 8 < p.n_rec;
-    fz_add_rows(v, valid0 ? rec + ra * 64 : nullptr, valid1 ? rec + (ra + 8) * 64 : nullptr);  // L2-hot since step 1
-    fz_store_op(sN, v, rq, wg);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int t = 0; t < 16; ++t) v[i][t] += res[i][t];
+    fz_store_op(sN, v, rq, c);
     fz_gemm(acc, aN, sb + dec::WO1, 2);
     fz_unpack(acc, v, prm + 448);
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
       for (int t = 0; t < 16; ++t) v[i][t] = silu_fast(v[i][t]);
-    fz_store_op(sN, v, rq, wg);
+    fz_store_op(sN, v, rq, c);
     fz_gemm(acc, aN, sb + dec::WO2, 2);
     fz_unpack(acc, v, prm + 512);
-    fz_store_rows(p, p.out, p.D, p.n_rec, true, v, b, ra, valid0, valid1);
+    const long long ra = r0 + lr;
+    fz_store_rows(p, p.out, p.D, p.n_rec, true, v, b, ra, ra < p.n_rec, ra + 8 < p.n_rec);
   }
 }
 
@@ -1948,7 +2034,7 @@ int tc_decode(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_m
                        4.0 * (7 * 64 * 64 + 64 * D + 9 * 64);
   {
     ProfScope ps("tc_decode_kernel", st, bytes);
-    kern<<<grid, fz::THREADS, dec::BYTES, st>>>(p);
+    kern<<<grid, dec::THREADS, dec::BYTES, st>>>(p);
   }
   count_launch();
   NLAM_CUDA_OK(cudaGetLastError());

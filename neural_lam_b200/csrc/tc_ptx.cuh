@@ -42,6 +42,23 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// mbar_wait without the diagnostic printf, for kernels whose MMAs must stay pipelined: a call (printf) anywhere in a kernel
+// makes ptxas wait for every wgmma before issuing the next (C7510)
+__device__ __forceinline__ void mbar_wait_nocall(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+  uint32_t spins = 0;
+  while (true) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(bar), "r"(parity), "r"(1000000u)
+        : "memory");
+    if (done) break;
+    if (++spins > (1u << 20)) __trap();  // bounded: a protocol bug must not hang the GPU
+  }
+}
 __device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
   uint32_t done;
   asm volatile(
@@ -142,6 +159,8 @@ __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* map, int c0, 
                ::"l"(map), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+// bring one 128-byte line into L2 without holding a register
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, uint64_t pol) {
   asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol) : "memory");
 }
