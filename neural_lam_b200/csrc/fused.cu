@@ -5,19 +5,16 @@
 //   h  = SiLU(A · W1ᵀ + b1)                                wgmma, accumulators in registers, h back to shared memory
 //   y  = LN(h · W2ᵀ + b2) [+ residual]                     wgmma
 //
-// then one of: the row output (optionally the forecast-step epilogue), the edge output e' = e + y together with the
-// deterministic per-receiver sum of y over the tile's edges (every receiver lies in one tile), or two more 64-wide GEMMs on
-// y (the next layer's node projections; or output_map and the step epilogue).  All weights of a launch stay in shared
-// memory for the whole persistent CTA; operands are written in the 128-byte swizzle wgmma reads, and every generic-proxy
-// write of an operand is followed by fence.proxy.async before the warp group's MMAs read it.
+// then one of: the row output (optionally the forecast-step epilogue), or the edge output e' = e + y together with the
+// deterministic per-receiver sum of y over the tile's edges (every receiver lies in one tile).  All weights of a launch
+// stay in shared memory for the whole persistent CTA; operands are written in the 128-byte swizzle wgmma reads, and every
+// generic-proxy write of an operand is followed by fence.proxy.async before the warp group's MMAs read it.
 //
-// Launch names (nlam_profile_*): tc_rowmlp_kernel (row MLPs, node updates, output_map + step epilogue),
-// tc_rowlinear_kernel (node projections P_s = x_s·W1sᵀ, P_r = x_r·W1rᵀ + b1 of the split first edge Linear, both node
-// sets in one grid), tc_edge_kernel (K = 192 edge MLP on raw gathered rows), tc_node_proj_kernel (node update + next layer's projections), tc_node_out_kernel (node update + output_map + step
-// epilogue), tc_decode_kernel (the whole mesh -> grid decoder of a forecast step, see below).  The node updates
-// (tc_node_proj_kernel, tc_node_out_kernel and the node-update form of tc_rowmlp_kernel) run on tc_node_kernel below, which
-// does this kernel's arithmetic with the next rows staged while the current ones compute; fused_mlp_kernel keeps them as the
-// fallback (node_pipelined).  The split-form edge stage
+// Launch names (nlam_profile_*): tc_rowmlp_kernel (row MLPs, output_map + step epilogue), tc_rowlinear_kernel (node
+// projections P_s = x_s·W1sᵀ, P_r = x_r·W1rᵀ + b1 of the split first edge Linear, both node sets in one grid), tc_edge_kernel
+// (K = 192 edge MLP on raw gathered rows).  The other kernels of this file each run one job: the node updates
+// (tc_node_proj_kernel, tc_node_out_kernel and the node-update form of tc_rowmlp_kernel) run on tc_node_kernel, the whole
+// mesh -> grid decoder of a forecast step on tc_decode_kernel.  The split-form edge stage
 // (first edge Linear split into e·W1eᵀ and node projections gathered in its epilogue) runs in tc_edge_split_kernel below
 // (tc_edge_split).  tc_edge_path decides, in one place, whether an edge stage takes the split or the K = 192 form and under
 // which label the split kernel is launched: tc_edge3_kernel (out-of-place edge output), tc_edge_rmw_kernel (edge tensor
@@ -33,25 +30,23 @@ constexpr int THREADS = 256;
 constexpr uint32_t CH_A = 128 * 128;  // one 32-column chunk of a 128-row operand
 constexpr uint32_t CH_W = 64 * 128;   // one 32-column chunk of a 64-row weight
 constexpr uint32_t OFF_A = 0;
+enum Mode { ROWS = 0, EDGE = 1, ROWLIN = 2 };
 // Shared memory, sized per launch so that the K = 64 launches fit two CTAs per SM:
-//   A (max(kc1, 2) chunks) | W1 (kc1 chunks) | W2 (2) | W3, W4 (2 + 2; for the edge modes the 128 x 64 fp32 message buffer)
-//   | b1 | b2 | gamma | beta | b3 | b4 | b1 of problem 1 (64 floats each)
+//   A (max(kc1, 2) chunks) | W1 (kc1 chunks) | W2 (2) | EDGE: the 128 x 64 fp32 message buffer, ROWLIN: W3 (2)
+//   | b1 | b2 | gamma | beta | b1 of problem 1 (64 floats each, in a block of 7: the launch sizes, and with them the CTAs
+//   per SM, are those the kernel was tuned and measured at)
 struct Layout {
-  uint32_t w1, w2, w3, w4, prm, bytes;
+  uint32_t w1, w2, w3, prm, bytes;
 };
-__host__ __device__ inline Layout layout(int kc1, int mode, int post) {
+__host__ __device__ inline Layout layout(int kc1, int mode) {
   Layout l;
   l.w1 = (uint32_t)(kc1 > 2 ? kc1 : 2) * CH_A;
   l.w2 = l.w1 + (uint32_t)kc1 * CH_W;
   l.w3 = l.w2 + 2 * CH_W;
-  l.w4 = l.w3 + 2 * CH_W;
-  const uint32_t tail = (post != 0 || mode == 1) ? 4 * CH_W : (mode == 2 ? 2 * CH_W : 0);
-  l.prm = l.w3 + tail;
+  l.prm = l.w3 + (mode == EDGE ? 4 * CH_W : mode == ROWLIN ? 2 * CH_W : 0);
   l.bytes = l.prm + 7 * 64 * 4 + 1024;  // + alignment slack
   return l;
 }
-enum Mode { ROWS = 0, EDGE = 1, ROWLIN = 2 };
-enum Post { POST_NONE = 0, POST_PROJ = 1, POST_OUTMLP = 2 };
 }  // namespace fz
 
 struct FzSrc {
@@ -66,10 +61,10 @@ struct FzW {           // rows x cols slice of a row-major matrix with row pitch
 };
 
 struct FzParams {
-  int mode, post, B, kc1, n_src;
+  int mode, B, kc1, n_src;
   FzSrc src[4];
-  FzW w1, w2, w3, w4;
-  const float *b1, *b2, *gamma, *beta, *b3, *b4;
+  FzW w1, w2, w3;
+  const float *b1, *b2, *gamma, *beta;
   float eps;
   int act1, has_gemm2;
   const float* res;     // residual rows (64 wide)
@@ -87,9 +82,6 @@ struct FzParams {
   float* edge_out;      // (B, n_edges, 64) dense
   float* aggr;          // (B, n_rec, 64) dense
   long long n_rec, n_edges;
-  // POST_PROJ: out3 (B, n_rows, 64) = y·W3ᵀ, out4 = y·W4ᵀ + b4; POST_OUTMLP: y -> SiLU(y·W3ᵀ + b3) -> ·W4ᵀ + b4 -> step
-  float* out3;
-  float* out4;
   // forecast-step epilogue on the final narrow output (width out_w)
   int step;
   const float *prev, *bnd, *mask, *dstd, *dmean;
@@ -276,8 +268,8 @@ __device__ __forceinline__ void fz_store_rows(const P& p, float* out, int W, lon
 
 __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_constant__ FzParams p) {
   using namespace fz;
-  const Layout L = layout(p.kc1, p.mode, p.post);
-  const uint32_t OFF_W1 = L.w1, OFF_W2 = L.w2, OFF_W3 = L.w3, OFF_W4 = L.w4, OFF_PRM = L.prm;
+  const Layout L = layout(p.kc1, p.mode);
+  const uint32_t OFF_W1 = L.w1, OFF_W2 = L.w2, OFF_W3 = L.w3, OFF_PRM = L.prm;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* s = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const uint32_t sb = smem_u32(s);
@@ -289,16 +281,13 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
 
   fz_load_w(s + OFF_W1, p.w1, p.kc1, tid);
   if (p.has_gemm2) fz_load_w(s + OFF_W2, p.w2, 2, tid);
-  if (p.post != POST_NONE || p.mode == ROWLIN) fz_load_w(s + OFF_W3, p.w3, 2, tid);
-  if (p.post != POST_NONE) fz_load_w(s + OFF_W4, p.w4, 2, tid);
+  if (p.mode == ROWLIN) fz_load_w(s + OFF_W3, p.w3, 2, tid);
   for (int i = tid; i < 64; i += THREADS) {
     prm[i] = p.b1 ? p.b1[i] : 0.f;
     prm[64 + i] = p.b2 ? p.b2[i] : 0.f;
     prm[128 + i] = p.gamma ? p.gamma[i] : 1.f;
     prm[192 + i] = p.beta ? p.beta[i] : 0.f;
-    prm[256 + i] = p.b3 ? p.b3[i] : 0.f;
-    prm[320 + i] = p.b4 ? p.b4[i] : 0.f;
-    prm[384 + i] = p.b1_1 ? p.b1_1[i] : 0.f;
+    prm[256 + i] = p.b1_1 ? p.b1_1[i] : 0.f;
   }
   const long long n_work0 = (long long)p.n_tiles * p.B;
   const long long n_work = n_work0 + (p.mode == ROWLIN ? (long long)p.n_tiles1 * p.B1 : 0);
@@ -336,7 +325,7 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
     fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + (prob ? OFF_W3 : OFF_W1), p.kc1);
     const long long r0 = row0 + rq;
     const bool valid0 = rq < nrows, valid1 = rq + 8 < nrows;
-    fz_unpack(acc, v, prm + (prob ? 384 : 0));
+    fz_unpack(acc, v, prm + (prob ? 256 : 0));
     if (p.mode == ROWLIN) {
       fz_store_rows(p, prob ? p.out_1 : p.out, 64, prob ? p.n_rows1 : p.n_rows, false, v, b, r0, valid0, valid1);
       continue;
@@ -396,33 +385,7 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
       const float* base = p.res + (long long)b * p.res_bs;
       fz_add_rows(v, valid0 ? base + r0 * 64 : nullptr, valid1 ? base + (r0 + 8) * 64 : nullptr);
     }
-    if (p.post == POST_NONE) {
-      fz_store_rows(p, p.out, p.out_w, p.n_rows, p.step, v, b, r0, valid0, valid1);
-      continue;
-    }
-    if (p.post == POST_PROJ) {
-      fz_store_rows(p, p.out, 64, p.n_rows, false, v, b, r0, valid0, valid1);  // the updated node rows
-      fz_store_op(sA, v, rq, wg);
-      fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W3, 2);
-      fz_unpack(acc, v, nullptr);
-      fz_store_rows(p, p.out3, 64, p.n_rows, false, v, b, r0, valid0, valid1);
-      fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W4, 2);
-      fz_unpack(acc, v, prm + 320);
-      fz_store_rows(p, p.out4, 64, p.n_rows, false, v, b, r0, valid0, valid1);
-      continue;
-    }
-    // POST_OUTMLP: the updated node rows stay on chip
-    fz_store_op(sA, v, rq, wg);
-    fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W3, 2);
-    fz_unpack(acc, v, prm + 256);
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int t2 = 0; t2 < 16; ++t2) v[i][t2] = silu_fast(v[i][t2]);
-    fz_store_op(sA, v, rq, wg);
-    fz_gemm(acc, sb + OFF_A + wg * (CH_A / 2), sb + OFF_W4, 2);
-    fz_unpack(acc, v, prm + 320);
-    fz_store_rows(p, p.out, p.out_w, p.n_rows, true, v, b, r0, valid0, valid1);
+    fz_store_rows(p, p.out, p.out_w, p.n_rows, p.step, v, b, r0, valid0, valid1);
   }
 }
 
@@ -914,8 +877,8 @@ __global__ void __launch_bounds__(dec::THREADS, 1) tc_decode_kernel(const __grid
     }
     fence_proxy_async();
     named_bar_sync(bar, 128);
-    // ---- 3. node MLP on [rec | aggr] (chunks 2-3 of Wn1 on aggr) + residual, output_map, step epilogue (as the
-    // POST_OUTMLP path of tc_node_kernel)
+    // ---- 3. node MLP on [rec | aggr] (chunks 2-3 of Wn1 on aggr) + residual, output_map, step epilogue (as in
+    // tc_node_out_kernel)
     dec_gemm_add(acc1, aN, sb + dec::WN1 + 2 * CH_W, 2);
     fz_unpack(acc1, v, prm + 192);
 #pragma unroll
@@ -1327,13 +1290,14 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_latent_kernel(const __grid_
 
 // ------------------------------------------------------------------------------------ H = 64 node update
 // The node update of an InteractionNet layer, out = res + LN(SiLU([src_0 | src_1]·Wn1ᵀ + bn1)·Wn2ᵀ + bn2) with res one of the
-// two 64-wide sources (rec for InteractionNet, aggr for PropagationNet), followed by one of fused_mlp_kernel's epilogues:
+// two 64-wide sources (rec for InteractionNet, aggr for PropagationNet), followed by one of three epilogues:
 //   POST_NONE    out                                                  (tc_rowmlp_kernel)
 //   POST_PROJ    out, P_s = out·W3ᵀ, P_r = out·W4ᵀ + b4               (tc_node_proj_kernel)
 //   POST_OUTMLP  step epilogue of SiLU(out·W3ᵀ + b3)·W4ᵀ + b4, out on chip   (tc_node_out_kernel)
-// The arithmetic is fused_mlp_kernel's, row for row: the same m64n64k8 MMAs in the same K order, the same TF32 rounding
-// points (operands rounded to nearest as they enter shared memory) and the same epilogue code, so the two kernels agree bit
-// for bit.  What differs is the load schedule.  Work items, warp-group ownership and staging are those of tc_latent_kernel:
+// Every GEMM is m64n64k8 MMAs over 64-row tiles on operands rounded to TF32 (to nearest) as they enter shared memory, with
+// the epilogue code of the row kernels above, so POST_PROJ's projections equal tc_rowlinear_kernel's on the same rows, and
+// POST_OUTMLP's output equals POST_NONE followed by fused_mlp_kernel's row MLP with the step epilogue, bit for bit.  Work
+// items, warp-group ownership and staging are those of tc_latent_kernel:
 // an item is 64 rows of one batch element and belongs to one warp group; the item's two source spans (64 x 256 B each,
 // contiguous and 16-byte aligned) are copied with cp.async into the warp group's raw staging rows while the previous item's
 // GEMMs run.  cp.async does not round, so staging -> operand applies tf32r4 as fz_load_a does; the residual is read from
@@ -1349,10 +1313,11 @@ constexpr uint32_t STG_WG = 2 * 64 * PITCH * 4;
 constexpr uint32_t PRM = STG + 2 * STG_WG;             // bn1 | bn2 | gamma | beta | b3 | b4
 constexpr uint32_t BYTES = PRM + 6 * 64 * 4 + 1024;    // + alignment slack
 static_assert(BYTES <= 227 * 1024, "node kernel shared memory exceeds the sm_90 limit");
+enum Post { POST_NONE = 0, POST_PROJ = 1, POST_OUTMLP = 2 };
 }  // namespace nod
 
 struct NodeParams {
-  int B, post, res_src;       // post: fz::Post; res_src: the source that is also the residual
+  int B, post, res_src;       // post: nod::Post; res_src: the source that is also the residual
   long long n_rows, n_tiles;  // rows; 64-row tiles per batch element
   const float* src[2];        // (B | 1, n_rows, 64), batch stride bs (0: shared by the batch)
   long long bs[2];
@@ -1383,11 +1348,11 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_node_kernel(const __grid_co
 
   fz_load_w(s + nod::WN1, p.wn1, 4, tid);
   fz_load_w(s + nod::WN2, p.wn2, 2, tid);
-  if (p.post != POST_NONE) {
+  if (p.post != nod::POST_NONE) {
     fz_load_w(s + nod::W3, p.w3, 2, tid);
     fz_load_w(s + nod::W4, p.w4, 2, tid);
   }
-  for (int i = tid; i < 64; i += THREADS) {  // the defaults of fused_mlp_kernel
+  for (int i = tid; i < 64; i += THREADS) {  // a Linear without bias adds zeros, a LayerNorm without beta too
     prm[i] = p.bn1 ? p.bn1[i] : 0.f;
     prm[64 + i] = p.bn2 ? p.bn2[i] : 0.f;
     prm[128 + i] = p.gamma[i];
@@ -1460,9 +1425,9 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_node_kernel(const __grid_co
       for (int t = 0; t < 16; ++t) v[i][t] += r[i][t];
     const long long r0 = row0 + lr;
     // ---- 3. epilogue
-    if (p.post == POST_NONE) {
+    if (p.post == nod::POST_NONE) {
       fz_store_rows(p, p.out, 64, p.n_rows, false, v, b, r0, valid0, valid1);
-    } else if (p.post == POST_PROJ) {
+    } else if (p.post == nod::POST_PROJ) {
       fz_store_rows(p, p.out, 64, p.n_rows, false, v, b, r0, valid0, valid1);  // the updated node rows
       fz_store_op(sA, v, rq, wg);
       fz_gemm(acc, aA, sb + nod::W3, 2);
@@ -1490,114 +1455,73 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_node_kernel(const __grid_co
 // ------------------------------------------------------------------------------------ host
 static FzW wslice(const float* w, int ld, int rows, int cols) { return FzW{w, ld, rows, cols}; }
 
+// One launch of the persistent kernel K over `items` work items (none: nothing to launch), `threads` threads and `smem`
+// bytes of dynamic shared memory per CTA.  K's dynamic shared-memory limit is raised to smem_limit once per device.  grid
+// is the CTA count; 0 asks for as many CTAs as fit on every SM at `smem` bytes, at most one per item, which the occupancy
+// calculator can tell only once the limit is raised.
+template <auto K, class P>
+static int persistent_launch(int threads, size_t smem, size_t smem_limit, long long items, int grid, const char* name,
+                             double bytes, cudaStream_t st, const P& p) {
+  if (items == 0) return NLAM_OK;
+  NLAM_REQUIRE(items < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
+  int dev = 0;
+  NLAM_CUDA_OK(cudaGetDevice(&dev));
+  static unsigned optin = 0;  // one bit per device on which K's limit is raised
+  if (!(optin & (1u << (dev & 31)))) {
+    NLAM_CUDA_OK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit));
+    optin |= 1u << (dev & 31);
+  }
+  if (grid == 0) {
+    int per_sm = 1;
+    NLAM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, K, threads, smem));
+    grid = (int)std::min<long long>(items, (long long)num_sms() * std::max(per_sm, 1));
+  }
+  {
+    ProfScope ps(name, st, bytes);
+    K<<<grid, threads, smem, st>>>(p);
+  }
+  count_launch();
+  NLAM_CUDA_OK(cudaGetLastError());
+  return NLAM_OK;
+}
+
+// fused_mlp_kernel: as many CTAs per SM as fit (two for the K = 64 launches); the limit covers the largest layout
 static int fz_launch(const FzParams& p, const char* name, double bytes, cudaStream_t st) {
   const long long n_work = (long long)p.n_tiles * p.B + (p.mode == fz::ROWLIN ? (long long)p.n_tiles1 * p.B1 : 0);
-  if (n_work == 0) return NLAM_OK;
-  NLAM_REQUIRE(n_work < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
-  int dev = 0;
-  NLAM_CUDA_OK(cudaGetDevice(&dev));
-  const size_t smem = fz::layout(p.kc1, p.mode, p.post).bytes;
-  static unsigned mask = 0;
-  if (!(mask & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(fused_mlp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)fz::layout(6, fz::EDGE, 0).bytes));
-    mask |= 1u << (dev & 31);
-  }
-  int per_sm = 1;
-  NLAM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fused_mlp_kernel, fz::THREADS, smem));
-  const int grid = (int)std::min<long long>(n_work, (long long)num_sms() * std::max(per_sm, 1));
-  {
-    ProfScope ps(name, st, bytes);
-    fused_mlp_kernel<<<grid, fz::THREADS, smem, st>>>(p);
-  }
-  count_launch();
-  NLAM_CUDA_OK(cudaGetLastError());
-  return NLAM_OK;
+  return persistent_launch<fused_mlp_kernel>(fz::THREADS, fz::layout(p.kc1, p.mode).bytes, fz::layout(6, fz::EDGE).bytes, n_work,
+                                             0, name, bytes, st, p);
 }
 
-// Whether the node update p (fz_node's two 64-wide sources, a residual equal to one of them, LayerNorm, out_w 64 or a step
-// epilogue) runs on tc_node_kernel: both sources 16-byte aligned with batch strides % 4 == 0 (one aligned cp.async span per
-// item), unless NLAM_TC_NODE=v1 asks for fused_mlp_kernel.  Read at every call, so that one process can run both kernels on
-// the same inputs; the two agree bit for bit.
-static bool node_pipelined(const FzParams& p) {
-  const char* e = getenv("NLAM_TC_NODE");
-  if (e && e[0] == 'v' && e[1] == '1') return false;
-  for (int q = 0; q < 2; ++q)
-    if (!aligned16(p.src[q].ptr) || p.src[q].bs % 4 != 0) return false;
-  return true;
-}
-
-static int node_launch(const FzParams& f, int res_src, const char* name, double bytes, cudaStream_t st) {
+// The node update every tc_node_kernel launch starts with: [src_0 | src_1] (64 wide each, batch strides bs0 / bs1) through a
+// node MLP (node_mlp_ok), plus source res_src as the residual, into out (B, n_rows, 64) unless the epilogue keeps it
+static NodeParams node_params(const NlamMlp* m, const float* src0, int64_t bs0, const float* src1, int64_t bs1, int res_src,
+                              int64_t n_rows, int B, float* out) {
   NodeParams p;
   memset(&p, 0, sizeof(p));
-  p.B = f.B;
-  p.post = f.post;
+  p.B = B;
   p.res_src = res_src;
-  p.n_rows = f.n_rows;
-  p.n_tiles = (f.n_rows + 63) / 64;
-  for (int q = 0; q < 2; ++q) {
-    p.src[q] = f.src[q].ptr;
-    p.bs[q] = f.src[q].bs;
-  }
-  p.wn1 = f.w1;
-  p.wn2 = f.w2;
-  p.w3 = f.w3;
-  p.w4 = f.w4;
-  p.bn1 = f.b1;
-  p.bn2 = f.b2;
-  p.gamma = f.gamma;
-  p.beta = f.beta;
-  p.b3 = f.b3;
-  p.b4 = f.b4;
-  p.eps = f.eps;
-  p.out = f.out;
-  p.out_w = f.out_w;
-  p.out3 = f.out3;
-  p.out4 = f.out4;
-  p.prev = f.prev;
-  p.bnd = f.bnd;
-  p.mask = f.mask;
-  p.dstd = f.dstd;
-  p.dmean = f.dmean;
-  const long long n_items = p.n_tiles * p.B;
-  if (n_items == 0) return NLAM_OK;
-  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
-  int dev = 0;
-  NLAM_CUDA_OK(cudaGetDevice(&dev));
-  static unsigned mask = 0;
-  if (!(mask & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_node_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nod::BYTES));
-    mask |= 1u << (dev & 31);
-  }
-  const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
-  {
-    ProfScope ps(name, st, bytes);
-    tc_node_kernel<<<grid, fz::THREADS, nod::BYTES, st>>>(p);
-  }
-  count_launch();
-  NLAM_CUDA_OK(cudaGetLastError());
-  return NLAM_OK;
+  p.n_rows = n_rows;
+  p.n_tiles = (n_rows + 63) / 64;
+  p.src[0] = src0;
+  p.src[1] = src1;
+  p.bs[0] = B > 1 ? bs0 : 0;
+  p.bs[1] = B > 1 ? bs1 : 0;
+  p.wn1 = wslice(m->w[0], 128, 64, 128);
+  p.wn2 = wslice(m->w[1], 64, 64, 64);
+  p.bn1 = m->b[0];
+  p.bn2 = m->b[1];
+  p.gamma = m->ln_gamma;
+  p.beta = m->ln_beta;
+  p.eps = m->ln_eps;
+  p.out = out;
+  p.out_w = 64;
+  return p;
 }
 
-static int edge_split_launch(const EdgeParams& p, const char* name, double bytes, cudaStream_t st) {
-  const long long n_work = (long long)p.n_tiles * p.B;
-  if (n_work == 0) return NLAM_OK;
-  NLAM_REQUIRE(n_work < (1LL << 40), NLAM_E_INVALID, "%s: bad work size", name);
-  int dev = 0;
-  NLAM_CUDA_OK(cudaGetDevice(&dev));
-  static unsigned mask = 0;
-  if (!(mask & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_edge_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)edg::BYTES));
-    mask |= 1u << (dev & 31);
-  }
-  const int grid = (int)std::min<long long>(n_work, num_sms());  // one CTA per SM
-  {
-    ProfScope ps(name, st, bytes);
-    tc_edge_split_kernel<<<grid, fz::THREADS, edg::BYTES, st>>>(p);
-  }
-  count_launch();
-  NLAM_CUDA_OK(cudaGetLastError());
-  return NLAM_OK;
+static int node_launch(const NodeParams& p, const char* name, double bytes, cudaStream_t st) {
+  const long long n_items = p.n_tiles * p.B;
+  const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
+  return persistent_launch<tc_node_kernel>(fz::THREADS, nod::BYTES, nod::BYTES, n_items, grid, name, bytes, st, p);
 }
 
 static void fz_mlp(FzParams& p, const NlamMlp* m, int k_off, int k_cols) {
@@ -1654,27 +1578,32 @@ int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamR
   const int nout = mlp->out_dim[1];
   NLAM_REQUIRE(!ep || (nout < 64 && !mlp->ln_gamma && !res), NLAM_E_UNSUPPORTED,
                "tc_rowmlp: the fused step epilogue needs a narrow output without LayerNorm / residual");
+  double bytes = 0;
+  for (int s = 0; s < n_src; ++s) bytes += 4.0 * n_rows * srcs[s].dim * ((srcs[s].bstride != 0 && B > 1) ? B : 1);
+  if (res) bytes += 4.0 * n_rows * 64 * ((res->bstride != 0 && B > 1) ? B : 1);
+  bytes += 4.0 * n_rows * B * nout;
+  if (ep) bytes += 4.0 * n_rows * B * nout * (ep->boundary ? 2 : 1);
+  // node update: two 64-wide sources, the residual one of them
+  if (res && !ep && n_src == 2 && srcs[0].dim == 64 && srcs[1].dim == 64 && node_mlp_ok(mlp)) {
+    const int res_src = (srcs[0].ptr == res->ptr && srcs[0].bstride == res->bstride) ? 0 : 1;
+    return node_launch(node_params(mlp, srcs[0].ptr, srcs[0].bstride, srcs[1].ptr, srcs[1].bstride, res_src, n_rows, B, out),
+                       "tc_rowmlp_kernel", bytes, st);
+  }
   FzParams p;
   memset(&p, 0, sizeof(p));
   p.mode = fz::ROWS;
   p.B = B;
   p.n_src = n_src;
-  double bytes = 0;
-  for (int s = 0; s < n_src; ++s) {
-    p.src[s] = FzSrc{srcs[s].ptr, srcs[s].idx, B > 1 ? srcs[s].bstride : 0, srcs[s].dim};
-    bytes += 4.0 * n_rows * srcs[s].dim * ((srcs[s].bstride != 0 && B > 1) ? B : 1);
-  }
+  for (int s = 0; s < n_src; ++s) p.src[s] = FzSrc{srcs[s].ptr, srcs[s].idx, B > 1 ? srcs[s].bstride : 0, srcs[s].dim};
   fz_mlp(p, mlp, 0, mlp->in_dim);
   if (res) {
     p.res = res->ptr;
     p.res_bs = B > 1 ? res->bstride : 0;
-    bytes += 4.0 * n_rows * 64 * ((res->bstride != 0 && B > 1) ? B : 1);
   }
   p.out = out;
   p.out_w = nout;
   p.n_rows = n_rows;
   p.n_tiles = (int)((n_rows + 127) / 128);
-  bytes += 4.0 * n_rows * B * nout;
   if (ep) {
     p.step = 1;
     p.prev = ep->prev;
@@ -1682,13 +1611,7 @@ int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamR
     p.mask = ep->mask;
     p.dstd = ep->std;
     p.dmean = ep->mean;
-    bytes += 4.0 * n_rows * B * nout * (ep->boundary ? 2 : 1);
   }
-  // node update: two 64-wide sources, the residual one of them
-  int res_src = -1;
-  if (res && !ep && n_src == 2 && srcs[0].dim == 64 && srcs[1].dim == 64 && node_mlp_ok(mlp))
-    res_src = (srcs[0].ptr == res->ptr && srcs[0].bstride == res->bstride) ? 0 : 1;
-  if (res_src >= 0 && node_pipelined(p)) return node_launch(p, res_src, "tc_rowmlp_kernel", bytes, st);
   return fz_launch(p, "tc_rowmlp_kernel", bytes, st);
 }
 
@@ -1734,23 +1657,12 @@ static bool tc_edge_supported(const NlamGraph* g, const NlamMlp* edge_mlp, int f
   return true;
 }
 
-static int edge_mode_env() {
-  // NLAM_TC_EDGE=v1 | v2 forces one formulation of the first edge Linear (rule 2 of tc_edge_path)
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("NLAM_TC_EDGE");
-    mode = (e && e[0] == 'v' && e[1] == '1') ? 1 : (e && e[0] == 'v' && e[1] == '2') ? 2 : 0;
-  }
-  return mode;
-}
-
 // Which form and launch label an edge stage takes: the first rule that applies (DESIGN.md §4.1).  The split form and the
 // K = 192 form round differently in TF32, and only tc_edge_rmw_kernel may write its edge output over its edge input, so the
 // dispatch and every support query in abi.cu ask here.
 //   1. no edge output, uniform in-degree 1..8: split, tc_ell_window_kernel, always with its own projection pass
-//   2. NLAM_TC_EDGE=v2, or (unless v1) E·B >= 2.5·(n_send·Bs + n_rec·Br): the projection pass is small next to the edge
-//      work (mesh graphs): split, tc_edge_rmw_kernel without edge output or with it over a dense edge input, else
-//      tc_edge3_kernel
+//   2. E·B >= 2.5·(n_send·Bs + n_rec·Br): the projection pass is small next to the edge work (mesh graphs): split,
+//      tc_edge_rmw_kernel without edge output or with it over a dense edge input, else tc_edge3_kernel
 //   3. no edge output, edge features and receivers shared by the batch (grid -> mesh): split, tc_edge_bcast_kernel; both
 //      projections are far fewer rows than the batch's edges
 //   4. otherwise: K = 192 on raw gathered rows, tc_edge_kernel
@@ -1761,11 +1673,10 @@ TcEdgePath tc_edge_path(const NlamGraph* g, const NlamMlp* edge_mlp, int flags, 
   if (!tc_edge_supported(g, edge_mlp, flags)) return {};
   const bool aligned = aligned16(send) && aligned16(rec) && send_bs % 4 == 0 && rec_bs % 4 == 0;
   if (!edge_out && g->uniform_degree >= 1 && g->uniform_degree <= 8 && aligned) return {"tc_ell_window_kernel", true, false};
-  const int mode = edge_mode_env();
   const double edge_rows = (double)g->n_edges * B;
   const double node_rows = (double)g->n_send * ((send_bs == 0 || B == 1) ? 1 : B) +
                            (double)g->n_rec * ((rec_bs == 0 || B == 1) ? 1 : B);
-  if (aligned && (mode == 2 || (mode != 1 && edge_rows >= 2.5 * node_rows))) {
+  if (aligned && edge_rows >= 2.5 * node_rows) {
     const bool rmw = !edge_out || (edge_out == edge && (B == 1 || edge_bs == g->n_edges * 64));
     return {rmw ? "tc_edge_rmw_kernel" : "tc_edge3_kernel", true, true};
   }
@@ -1823,7 +1734,9 @@ static int fz_edge(const NlamGraph* g, const NlamMlp* em, const float* send, int
     q.eps = em->ln_eps;
     q.n_rec = g->n_rec;
     q.n_edges = g->n_edges;
-    return edge_split_launch(q, name, bytes, st);
+    const long long n_work = (long long)q.n_tiles * B;
+    const int grid = (int)std::min<long long>(n_work, num_sms());  // one CTA per SM
+    return persistent_launch<tc_edge_split_kernel>(fz::THREADS, edg::BYTES, edg::BYTES, n_work, grid, name, bytes, st, q);
   }
   FzParams p;
   memset(&p, 0, sizeof(p));
@@ -1870,38 +1783,19 @@ bool tc_node_proj_supported(const NlamMlp* node_mlp, const NlamMlp* next_edge_ml
   return aligned16(rec) && aligned16(aggr) && aligned16(out) && aligned16(proj_out) && rec_bs % 4 == 0;
 }
 
-static void fz_node(FzParams& p, const NlamMlp* node_mlp, const float* rec, int64_t rec_bs, const float* aggr, int64_t n_rows,
-                    int B) {
-  p.mode = fz::ROWS;
-  p.B = B;
-  p.n_src = 2;
-  p.src[0] = FzSrc{rec, nullptr, B > 1 ? rec_bs : 0, 64};
-  p.src[1] = FzSrc{aggr, nullptr, B > 1 ? n_rows * 64 : 0, 64};
-  fz_mlp(p, node_mlp, 0, 128);
-  p.res = rec;
-  p.res_bs = B > 1 ? rec_bs : 0;
-  p.n_rows = n_rows;
-  p.n_tiles = (int)((n_rows + 127) / 128);
-}
-
 int tc_node_proj(const NlamMlp* node_mlp, const NlamMlp* next_edge_mlp, const float* rec, int64_t rec_bs, const float* aggr,
                  int64_t n_rows, int B, float* out, float* proj_out, cudaStream_t st) {
   NLAM_REQUIRE(tc_node_proj_supported(node_mlp, next_edge_mlp, rec, rec_bs, aggr, n_rows, out, proj_out), NLAM_E_UNSUPPORTED,
                "tc_node_proj: unsupported shapes");
-  FzParams p;
-  memset(&p, 0, sizeof(p));
-  fz_node(p, node_mlp, rec, rec_bs, aggr, n_rows, B);
-  p.post = fz::POST_PROJ;
-  p.out = out;
-  p.out_w = 64;
+  NodeParams p = node_params(node_mlp, rec, rec_bs, aggr, n_rows * 64, 0, n_rows, B, out);
+  p.post = nod::POST_PROJ;
   p.w3 = wslice(next_edge_mlp->w[0] + 64, 192, 64, 64);
   p.w4 = wslice(next_edge_mlp->w[0] + 128, 192, 64, 64);
   p.b4 = next_edge_mlp->b[0];
   p.out3 = proj_out;
   p.out4 = proj_out + (size_t)B * n_rows * 64;
   const double bytes = 4.0 * n_rows * 64 * (((rec_bs != 0 && B > 1) ? B : 1) + 4.0 * B);
-  if (node_pipelined(p)) return node_launch(p, 0, "tc_node_proj_kernel", bytes, st);
-  return fz_launch(p, "tc_node_proj_kernel", bytes, st);
+  return node_launch(p, "tc_node_proj_kernel", bytes, st);
 }
 
 bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs, const float* aggr,
@@ -1918,26 +1812,21 @@ int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* re
                 int64_t n_rows, int B, float* out, const StepEpilogue* ep, cudaStream_t st) {
   NLAM_REQUIRE(tc_node_out_supported(node_mlp, out_mlp, rec, rec_bs, aggr, n_rows, B, out, ep), NLAM_E_UNSUPPORTED,
                "tc_node_out: unsupported shapes");
-  FzParams p;
-  memset(&p, 0, sizeof(p));
-  fz_node(p, node_mlp, rec, rec_bs, aggr, n_rows, B);
   const int D = out_mlp->out_dim[1];
-  p.post = fz::POST_OUTMLP;
+  NodeParams p = node_params(node_mlp, rec, rec_bs, aggr, n_rows * 64, 0, n_rows, B, out);
+  p.post = nod::POST_OUTMLP;
   p.w3 = wslice(out_mlp->w[0], 64, 64, 64);
   p.b3 = out_mlp->b[0];
   p.w4 = wslice(out_mlp->w[1], 64, D, 64);
   p.b4 = out_mlp->b[1];
-  p.out = out;
   p.out_w = D;
-  p.step = 1;
   p.prev = ep->prev;
   p.bnd = ep->boundary;
   p.mask = ep->mask;
   p.dstd = ep->std;
   p.dmean = ep->mean;
   const double bytes = 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + 3.0 * D * B);
-  if (node_pipelined(p)) return node_launch(p, 0, "tc_node_out_kernel", bytes, st);
-  return fz_launch(p, "tc_node_out_kernel", bytes, st);
+  return node_launch(p, "tc_node_out_kernel", bytes, st);
 }
 
 // ---- mesh -> grid decoder: edge projections (tc_rowlinear_kernel) + tc_decode_kernel
@@ -2015,30 +1904,17 @@ int tc_decode(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_m
   p.dstd = ep->std;
   p.dmean = ep->mean;
   const long long n_items = p.n_blocks * B;
-  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_decode: bad work size");
-  int dev = 0;
-  NLAM_CUDA_OK(cudaGetDevice(&dev));
-  void (*kern)(DecParams) = p.d == 1 ? tc_decode_kernel<1> : p.d == 2 ? tc_decode_kernel<2> : p.d == 4 ? tc_decode_kernel<4>
-                                                                                              : tc_decode_kernel<8>;
-  static unsigned mask[4] = {0, 0, 0, 0};
-  const int di = p.d == 1 ? 0 : p.d == 2 ? 1 : p.d == 4 ? 2 : 3;
-  if (!(mask[di] & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec::BYTES));
-    mask[di] |= 1u << (dev & 31);
-  }
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
   // algorithmic bytes: receivers, P_s, P_e and the sender indices once, previous / new (/ boundary) state, weights
   const int D = p.D, Br = (rec_bs != 0 && B > 1) ? B : 1;
   const double bytes = 256.0 * ((double)g->n_rec * Br + (double)g->n_send * Bs + (double)g->n_edges) + 4.0 * g->n_edges +
                        4.0 * (double)g->n_rec * D * B * (ep->boundary ? 3 : 2) + (ep->boundary ? 4.0 * g->n_rec : 0.0) +
                        4.0 * (7 * 64 * 64 + 64 * D + 9 * 64);
-  {
-    ProfScope ps("tc_decode_kernel", st, bytes);
-    kern<<<grid, dec::THREADS, dec::BYTES, st>>>(p);
-  }
-  count_launch();
-  NLAM_CUDA_OK(cudaGetLastError());
-  return NLAM_OK;
+  const auto launch = p.d == 1   ? persistent_launch<tc_decode_kernel<1>, DecParams>
+                      : p.d == 2 ? persistent_launch<tc_decode_kernel<2>, DecParams>
+                      : p.d == 4 ? persistent_launch<tc_decode_kernel<4>, DecParams>
+                                 : persistent_launch<tc_decode_kernel<8>, DecParams>;
+  return launch(dec::THREADS, dec::BYTES, dec::BYTES, n_items, grid, "tc_decode_kernel", bytes, st, p);
 }
 
 // ---- grid encoder: grid embedder + g2m node projections + encoding grid MLP (tc_encode_kernel)
@@ -2116,35 +1992,16 @@ int tc_encode(const NlamMlp* embed_mlp, const NlamRowSrc* srcs, int n_src, const
     p.pr_b = pr_b;
   }
   const long long n_items = p.n_tiles * B + (two ? 2 : 1) * p.n_mesh_tiles;
-  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_encode: bad work size");
-  int dev = 0;
-  NLAM_CUDA_OK(cudaGetDevice(&dev));
-  static unsigned mask = 0;
-  if (!(mask & (1u << (dev & 31)))) {
-    const int b1 = (int)enc::Layout<false>::BYTES, b2 = (int)enc::Layout<true>::BYTES;
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b1));
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b1));
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_encode_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2));
-    mask |= 1u << (dev & 31);
-  }
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
   // algorithmic bytes: the inputs once, grid_rep and P_s (and grid_emb or P_s_b), the mesh rows and P_r (and P_r_b), the
   // weights
   bytes += ((grid_emb || two) ? 3.0 : 2.0) * 4.0 * 64 * n_rows * B + (two ? 3.0 : 2.0) * 4.0 * 64 * n_mesh +
            4.0 * (embed_mlp->in_dim * 64 + (two ? 7 : 5) * 64 * 64 + (two ? 10 : 9) * 64);
-  if (two) {
-    ProfScope ps_("tc_encode2_kernel", st, bytes);
-    tc_encode_kernel<false, true><<<grid, fz::THREADS, enc::Layout<true>::BYTES, st>>>(p);
-  } else {
-    ProfScope ps_("tc_encode_kernel", st, bytes);
-    if (grid_emb)
-      tc_encode_kernel<true, false><<<grid, fz::THREADS, enc::Layout<false>::BYTES, st>>>(p);
-    else
-      tc_encode_kernel<false, false><<<grid, fz::THREADS, enc::Layout<false>::BYTES, st>>>(p);
-  }
-  count_launch();
-  NLAM_CUDA_OK(cudaGetLastError());
-  return NLAM_OK;
+  const size_t smem = two ? enc::Layout<true>::BYTES : enc::Layout<false>::BYTES;
+  const auto launch = two        ? persistent_launch<tc_encode_kernel<false, true>, EncParams>
+                      : grid_emb ? persistent_launch<tc_encode_kernel<true, false>, EncParams>
+                                 : persistent_launch<tc_encode_kernel<false, false>, EncParams>;
+  return launch(fz::THREADS, smem, smem, n_items, grid, two ? "tc_encode2_kernel" : "tc_encode_kernel", bytes, st, p);
 }
 
 // ---- Graph-EFM latent step: latent_param_map + sample + latent_embedder (tc_latent_kernel)
@@ -2191,24 +2048,10 @@ int tc_latent(const NlamMlp* param_mlp, const NlamMlp* embed_mlp, const float* x
   p.ln_eps = embed_mlp->ln_eps;
   p.out = out;
   const long long n_items = p.n_tiles * B;
-  NLAM_REQUIRE(n_items < (1LL << 40), NLAM_E_INVALID, "tc_latent: bad work size");
-  int dev = 0;
-  NLAM_CUDA_OK(cudaGetDevice(&dev));
-  static unsigned mask = 0;
-  if (!(mask & (1u << (dev & 31)))) {
-    NLAM_CUDA_OK(cudaFuncSetAttribute(tc_latent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lat::BYTES));
-    mask |= 1u << (dev & 31);
-  }
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
   // algorithmic bytes: x, eps and latent_emb once, the weights
   const double bytes = 3.0 * 4.0 * 64 * n_rows * B + 4.0 * ((p.diag ? 5 : 4) * 64 * 64 + (p.diag ? 8 : 7) * 64);
-  {
-    ProfScope ps_("tc_latent_kernel", st, bytes);
-    tc_latent_kernel<<<grid, fz::THREADS, lat::BYTES, st>>>(p);
-  }
-  count_launch();
-  NLAM_CUDA_OK(cudaGetLastError());
-  return NLAM_OK;
+  return persistent_launch<tc_latent_kernel>(fz::THREADS, lat::BYTES, lat::BYTES, n_items, grid, "tc_latent_kernel", bytes, st, p);
 }
 
 }  // namespace nlam

@@ -301,50 +301,30 @@ def test_model_rollout_tf32_vs_oracle(kind):
     torch.testing.assert_close(got_g, got, rtol=1e-6, atol=1e-6)
 
 
-def test_split_edge_kernel_v2_matches_v1_and_oracle():
-    """Both formulations of the first edge Linear — split (node projections + K=64 edge kernel, NLAM_TC_EDGE=v2) and K=192 with
-    raw gathered rows (tc.cu, NLAM_TC_EDGE=v1); forced in a fresh process, the selection is read once per process —
-    against the fp64 oracle."""
-    import os
-    import subprocess
-    import sys
-
-    code = r'''
-import os, sys, torch
-sys.path.insert(0, os.getcwd())
-import neural_lam_b200 as nlb
-from oracle import reference_port as rp
-g = torch.Generator().manual_seed(1)
-ns, nr, ne, B = 300, 300, 2600, 3
-ei = torch.stack([torch.randint(0, ns, (ne,), generator=g), torch.randint(0, nr, (ne,), generator=g)])
-ei[1, -1] = nr - 1
-ei = ei[:, torch.sort(ei[1], stable=True).indices]
-torch.manual_seed(0)
-res = {}
-for upd, aggr in ((True, "sum"), (False, "mean")):
-    net = nlb.InteractionNet(ei, 64, update_edges=upd, aggr=aggr, math="tf32")
-    send, edge = torch.randn(B, ns, 64), torch.randn(B, ne, 64)
-    want = rp.interaction_net({k: v.double() for k, v in net.state_dict().items()}, ei, send.double(), send.double(),
-                              edge.double(), aggr=aggr, update_edges=upd)
-    net = net.cuda()
-    with torch.no_grad():
-        got = net(send.cuda(), send.cuda(), edge.cuda())
-    got = got if isinstance(got, tuple) else (got,)
-    want = want if isinstance(want, tuple) else (want,)
-    err = max((a.double().cpu() - b).abs().max().item() for a, b in zip(got, want))
-    print("ERR", err)
-    assert err < 1e-2, err
-print("LAUNCHES", nlb._lib.lib().nlam_launch_count())
-'''
-    outs = {}
-    for mode, extra in (("v1", {}), ("v2", {})):
-        env = dict(os.environ, NLAM_TC_EDGE=mode, **extra)
-        r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env,
-                           cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))), timeout=300)
-        assert r.returncode == 0, r.stdout + r.stderr
-        outs[mode + ("_tc2" if extra else "")] = int([l for l in r.stdout.splitlines() if l.startswith("LAUNCHES")][0].split()[1])
-    # the split formulation issues one extra launch per InteractionNet call: both node projections in a single grid
-    assert outs["v2"] == outs["v1"] + 2
+def test_split_and_k192_edge_forms_vs_oracle():
+    """Both forms of the first edge Linear against the fp64 oracle, each picked by rule 2 of the edge path (DESIGN §4.1) on
+    graphs either side of its threshold at B = 3, ns = nr = 300 (2.5 x 1800 node rows = 4500 edge rows): split (node
+    projections in tc_rowlinear_kernel, then the K = 64 edge GEMM) for 2600 edges, K = 192 on raw gathered rows
+    (tc_edge_kernel) for 1000."""
+    B, ns, nr = 3, 300, 300
+    for ne, split in ((2600, True), (1000, False)):
+        ei = _graph(ns, nr, ne, 1, sort=True)
+        for upd, aggr in ((True, "sum"), (False, "mean")):
+            torch.manual_seed(0)
+            net = nlb.InteractionNet(ei, 64, update_edges=upd, aggr=aggr, math="tf32")
+            send, edge = torch.randn(B, ns, 64), torch.randn(B, ne, 64)
+            want = rp.interaction_net({k: v.double() for k, v in net.state_dict().items()}, ei, send.double(), send.double(),
+                                      edge.double(), aggr=aggr, update_edges=upd)
+            net = net.to(DEV)
+            with torch.no_grad(), ops.profile_launches() as prof:
+                got = net(send.to(DEV), send.to(DEV), edge.to(DEV))
+            edge_label = "tc_edge3_kernel" if upd else "tc_edge_rmw_kernel"
+            labels = ["tc_rowlinear_kernel", edge_label] if split else ["tc_edge_kernel"]
+            assert prof.names() == labels + ["tc_rowmlp_kernel"], (ne, upd, prof.names())
+            got = got if isinstance(got, tuple) else (got,)
+            want = want if isinstance(want, tuple) else (want,)
+            err = max((a.double().cpu() - b).abs().max().item() for a, b in zip(got, want))
+            assert err < 1e-2, (ne, upd, err)
 
 
 def _ell_graph(ns, nr, d, seed):
