@@ -179,6 +179,14 @@ int nlam_node_update_step_fwd(const NlamMlp* node_mlp, const NlamMlp* out_mlp, c
                               const float* aggr, const float* prev, const float* boundary, const float* bmask,
                               const float* diff_std, const float* diff_mean, float* new_state, int64_t n_rows, int B,
                               int flags, void* stream);
+/* The same for a model that predicts its std (reference --output_std, graph/base.py:322-344): out_mlp has 2·d outputs
+ * (2·d < 64) for d state variables.  Outputs 0..d-1 take the step epilogue above; std_out[b, r, c] = softplus(output d + c)
+ * (torch's threshold 20, not boundary-mixed).  prev, boundary, new_state and std_out are (B, n_rows, d) dense.
+ * NLAM_E_UNSUPPORTED where nlam_node_update_step_fwd would return it, or for an odd output count. */
+int nlam_node_update_step_std_fwd(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bstride,
+                                  const float* aggr, const float* prev, const float* boundary, const float* bmask,
+                                  const float* diff_std, const float* diff_mean, float* new_state, float* std_out,
+                                  int64_t n_rows, int B, int flags, void* stream);
 
 /* The whole mesh->grid decoder of a forecast step (reference gnn_layers.py:110-157 for the m2g InteractionNet, then
  * graph/base.py:322-342 and forecasters/autoregressive.py:128-131) in two launches (csrc/fused.cu): the edge projections
@@ -196,6 +204,13 @@ int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
                          int64_t edge_bstride, const float* prev, const float* boundary, const float* bmask,
                          const float* diff_std, const float* diff_mean, float* new_state, int B, int flags, void* workspace,
                          size_t ws_bytes, void* stream);
+/* The same for a model that predicts its std: out_mlp has 2·d outputs (2·d < 64), new_state and std_out (B, n_rec, d) as in
+ * nlam_node_update_step_std_fwd.  Same workspace. */
+int nlam_decode_step_std_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp,
+                             const float* send, int64_t send_bstride, const float* rec, int64_t rec_bstride, const float* edge,
+                             int64_t edge_bstride, const float* prev, const float* boundary, const float* bmask,
+                             const float* diff_std, const float* diff_mean, float* new_state, float* std_out, int B, int flags,
+                             void* workspace, size_t ws_bytes, void* stream);
 /* The grid side of a forecast step's encoder (reference graph/base.py:275-310) in one launch (csrc/fused.cu).  For the
  * concatenated inputs x = [src_0 | src_1 | ...] (at most 64 columns, dense rows without index) of each grid row:
  *   grid_emb = embed_mlp(x)                          never leaves the SM
@@ -382,6 +397,11 @@ int nlam_rowmlp_step_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, 
                          const float* boundary, const float* bmask, const float* diff_std,
                          const float* diff_mean, float* new_state, int64_t n_rows, int B, int flags,
                          void* stream);
+/* The same for a model that predicts its std: the MLP has 2·d outputs (2·d < 64); new_state and std_out (B, n_rows, d) as in
+ * nlam_node_update_step_std_fwd. */
+int nlam_rowmlp_step_std_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const float* prev, const float* boundary,
+                             const float* bmask, const float* diff_std, const float* diff_mean, float* new_state,
+                             float* std_out, int64_t n_rows, int B, int flags, void* stream);
 
 #ifdef __cplusplus
 }

@@ -120,6 +120,10 @@ SYMBOLS = {
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
         ctypes.c_void_p]),
+    "nlam_rowmlp_step_std_fwd": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
+        ctypes.c_void_p]),
     "nlam_step_epilogue_clamped": (ctypes.c_int, [ctypes.c_void_p] * 10 + [ctypes.c_int64] * 3 + [ctypes.c_void_p]),
     "nlam_halo_push": (ctypes.c_int, [
         ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
@@ -153,11 +157,20 @@ SYMBOLS = {
         ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int,
         ctypes.c_int, ctypes.c_void_p]),
+    "nlam_node_update_step_std_fwd": (ctypes.c_int, [
+        ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
+        ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "nlam_decode_workspace_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int]),
     "nlam_decode_step_fwd": (ctypes.c_int, [
         ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp),
         ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+        ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "nlam_decode_step_std_fwd": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamMlp),
+        ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "nlam_encode_supported": (ctypes.c_int, [
         ctypes.c_void_p, ctypes.POINTER(NlamMlp), ctypes.POINTER(NlamRowSrc), ctypes.c_int, ctypes.POINTER(NlamMlp),

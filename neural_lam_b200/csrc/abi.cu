@@ -37,31 +37,65 @@ extern "C" int nlam_rowmlp_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n
   return rowmlp_simt(mlp, srcs, n_src, res, res2, out, out2, n_rows, B, st);
 }
 
-extern "C" int nlam_rowmlp_step_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const float* prev,
-                                    const float* boundary, const float* bmask, const float* diff_std,
-                                    const float* diff_mean, float* new_state, int64_t n_rows, int B, int flags,
-                                    void* stream) {
+// The three fused step entries and their _std twins share one implementation each; std_out NULL: the plain step epilogue.
+static int rowmlp_step_impl(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const float* prev, const float* boundary,
+                            const float* bmask, const float* diff_std, const float* diff_mean, float* new_state, float* std_out,
+                            int64_t n_rows, int B, int flags, void* stream) {
   NLAM_REQUIRE(mlp && srcs && prev && diff_std && diff_mean && new_state, NLAM_E_INVALID, "nlam_rowmlp_step_fwd: null argument");
   NLAM_REQUIRE((boundary == nullptr) || bmask, NLAM_E_INVALID, "nlam_rowmlp_step_fwd: boundary without mask");
   const int nout = mlp->out_dim[mlp->n_linear - 1];
   // only the tensor-core path fuses the epilogue; callers fall back to nlam_rowmlp_fwd + nlam_step_epilogue
-  NLAM_REQUIRE(want_tf32(flags) && nout < 64 && !mlp->ln_gamma && tc_rowmlp_supported(mlp, srcs, n_src, nullptr, nullptr, n_rows),
+  NLAM_REQUIRE(want_tf32(flags) && nout < 64 && (!std_out || nout % 2 == 0) && !mlp->ln_gamma &&
+                   tc_rowmlp_supported(mlp, srcs, n_src, nullptr, nullptr, n_rows),
                NLAM_E_UNSUPPORTED, "nlam_rowmlp_step_fwd: shape / math mode not covered by the fused kernel");
-  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean};
+  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean, std_out};
   return tc_rowmlp(mlp, srcs, n_src, nullptr, new_state, n_rows, B, (cudaStream_t)stream, &ep);
+}
+
+extern "C" int nlam_rowmlp_step_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const float* prev,
+                                    const float* boundary, const float* bmask, const float* diff_std,
+                                    const float* diff_mean, float* new_state, int64_t n_rows, int B, int flags,
+                                    void* stream) {
+  return rowmlp_step_impl(mlp, srcs, n_src, prev, boundary, bmask, diff_std, diff_mean, new_state, nullptr, n_rows, B, flags,
+                          stream);
+}
+
+extern "C" int nlam_rowmlp_step_std_fwd(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const float* prev,
+                                        const float* boundary, const float* bmask, const float* diff_std, const float* diff_mean,
+                                        float* new_state, float* std_out, int64_t n_rows, int B, int flags, void* stream) {
+  NLAM_REQUIRE(std_out, NLAM_E_INVALID, "nlam_rowmlp_step_std_fwd: null std_out");
+  return rowmlp_step_impl(mlp, srcs, n_src, prev, boundary, bmask, diff_std, diff_mean, new_state, std_out, n_rows, B, flags,
+                          stream);
+}
+
+static int node_update_step_impl(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs,
+                                 const float* aggr, const float* prev, const float* boundary, const float* bmask,
+                                 const float* diff_std, const float* diff_mean, float* new_state, float* std_out, int64_t n_rows,
+                                 int B, int flags, void* stream) {
+  NLAM_REQUIRE(node_mlp && out_mlp && rec && aggr && prev && diff_std && diff_mean && new_state, NLAM_E_INVALID,
+               "nlam_node_update_step_fwd: null argument");
+  NLAM_REQUIRE((boundary == nullptr) || bmask, NLAM_E_INVALID, "nlam_node_update_step_fwd: boundary without mask");
+  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean, std_out};
+  NLAM_REQUIRE(want_tf32(flags) && tc_node_out_supported(node_mlp, out_mlp, rec, rec_bs, aggr, n_rows, B, new_state, &ep),
+               NLAM_E_UNSUPPORTED, "nlam_node_update_step_fwd: shape / math mode not covered by the fused kernel");
+  return tc_node_out(node_mlp, out_mlp, rec, rec_bs, aggr, n_rows, B, new_state, &ep, (cudaStream_t)stream);
 }
 
 extern "C" int nlam_node_update_step_fwd(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs,
                                          const float* aggr, const float* prev, const float* boundary, const float* bmask,
                                          const float* diff_std, const float* diff_mean, float* new_state, int64_t n_rows, int B,
                                          int flags, void* stream) {
-  NLAM_REQUIRE(node_mlp && out_mlp && rec && aggr && prev && diff_std && diff_mean && new_state, NLAM_E_INVALID,
-               "nlam_node_update_step_fwd: null argument");
-  NLAM_REQUIRE((boundary == nullptr) || bmask, NLAM_E_INVALID, "nlam_node_update_step_fwd: boundary without mask");
-  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean};
-  NLAM_REQUIRE(want_tf32(flags) && tc_node_out_supported(node_mlp, out_mlp, rec, rec_bs, aggr, n_rows, B, new_state, &ep),
-               NLAM_E_UNSUPPORTED, "nlam_node_update_step_fwd: shape / math mode not covered by the fused kernel");
-  return tc_node_out(node_mlp, out_mlp, rec, rec_bs, aggr, n_rows, B, new_state, &ep, (cudaStream_t)stream);
+  return node_update_step_impl(node_mlp, out_mlp, rec, rec_bs, aggr, prev, boundary, bmask, diff_std, diff_mean, new_state,
+                               nullptr, n_rows, B, flags, stream);
+}
+
+extern "C" int nlam_node_update_step_std_fwd(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* rec, int64_t rec_bs,
+                                             const float* aggr, const float* prev, const float* boundary, const float* bmask,
+                                             const float* diff_std, const float* diff_mean, float* new_state, float* std_out,
+                                             int64_t n_rows, int B, int flags, void* stream) {
+  NLAM_REQUIRE(std_out, NLAM_E_INVALID, "nlam_node_update_step_std_fwd: null std_out");
+  return node_update_step_impl(node_mlp, out_mlp, rec, rec_bs, aggr, prev, boundary, bmask, diff_std, diff_mean, new_state,
+                               std_out, n_rows, B, flags, stream);
 }
 
 static size_t rup256(size_t n) { return (n + 255) / 256 * 256; }
@@ -71,15 +105,15 @@ extern "C" size_t nlam_decode_workspace_bytes(const NlamGraph* g, int B) {
   return rup256(tc_decode_workspace_floats(g, B) * sizeof(float));
 }
 
-extern "C" int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp,
-                                    const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge,
-                                    int64_t edge_bs, const float* prev, const float* boundary, const float* bmask,
-                                    const float* diff_std, const float* diff_mean, float* new_state, int B, int flags,
-                                    void* workspace, size_t ws_bytes, void* stream) {
+static int decode_step_impl(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp,
+                            const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge, int64_t edge_bs,
+                            const float* prev, const float* boundary, const float* bmask, const float* diff_std,
+                            const float* diff_mean, float* new_state, float* std_out, int B, int flags, void* workspace,
+                            size_t ws_bytes, void* stream) {
   NLAM_REQUIRE(g && edge_mlp && node_mlp && out_mlp && send && rec && edge && prev && diff_std && diff_mean && new_state,
                NLAM_E_INVALID, "nlam_decode_step_fwd: null argument");
   NLAM_REQUIRE((boundary == nullptr) || bmask, NLAM_E_INVALID, "nlam_decode_step_fwd: boundary without mask");
-  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean};
+  StepEpilogue ep = {prev, boundary, bmask, diff_std, diff_mean, std_out};
   NLAM_REQUIRE(want_tf32(flags) && tc_decode_supported(g, edge_mlp, node_mlp, out_mlp, flags, send, send_bs, rec, rec_bs, edge,
                                                        edge_bs, B, new_state, &ep),
                NLAM_E_UNSUPPORTED, "nlam_decode_step_fwd: graph / shape / math mode not covered by the fused decoder");
@@ -88,6 +122,26 @@ extern "C" int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp,
                nlam_decode_workspace_bytes(g, B));
   return tc_decode(g, edge_mlp, node_mlp, out_mlp, flags, send, send_bs, rec, rec_bs, edge, edge_bs, B, new_state, &ep,
                    (float*)workspace, (cudaStream_t)stream);
+}
+
+extern "C" int nlam_decode_step_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp, const NlamMlp* out_mlp,
+                                    const float* send, int64_t send_bs, const float* rec, int64_t rec_bs, const float* edge,
+                                    int64_t edge_bs, const float* prev, const float* boundary, const float* bmask,
+                                    const float* diff_std, const float* diff_mean, float* new_state, int B, int flags,
+                                    void* workspace, size_t ws_bytes, void* stream) {
+  return decode_step_impl(g, edge_mlp, node_mlp, out_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, prev, boundary, bmask,
+                          diff_std, diff_mean, new_state, nullptr, B, flags, workspace, ws_bytes, stream);
+}
+
+extern "C" int nlam_decode_step_std_fwd(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_mlp,
+                                        const NlamMlp* out_mlp, const float* send, int64_t send_bs, const float* rec,
+                                        int64_t rec_bs, const float* edge, int64_t edge_bs, const float* prev,
+                                        const float* boundary, const float* bmask, const float* diff_std, const float* diff_mean,
+                                        float* new_state, float* std_out, int B, int flags, void* workspace, size_t ws_bytes,
+                                        void* stream) {
+  NLAM_REQUIRE(std_out, NLAM_E_INVALID, "nlam_decode_step_std_fwd: null std_out");
+  return decode_step_impl(g, edge_mlp, node_mlp, out_mlp, send, send_bs, rec, rec_bs, edge, edge_bs, prev, boundary, bmask,
+                          diff_std, diff_mean, new_state, std_out, B, flags, workspace, ws_bytes, stream);
 }
 
 // Workspace layout: [aggregate | path-specific scratch].  Sized per path: the fused H = 64 kernels need only the node

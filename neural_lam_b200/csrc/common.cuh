@@ -55,6 +55,7 @@ struct StepEpilogue {  // fused forecast-step epilogue of a narrow-output row ML
   const float* mask;
   const float* std;
   const float* mean;
+  float* std_out = nullptr;  // predicted-std form: the MLP has 2·d outputs, std_out (B, rows, d) = softplus(outputs d..2d-1)
 };
 // tc7.cu: generic wgmma Linear (any K multiple of 32, N <= 256) and the layer paths built from it
 struct LinearCall {

@@ -91,6 +91,7 @@ struct FzParams {
   float* out_1;
   long long n_rows1;
   int n_tiles1, B1;
+  float* std_out;       // predicted-std form of the step epilogue (fused_mlp_kernel<true>): (B, n_rows, out_w / 2)
 };
 
 // byte offset of operand element (row R, column c) in a 128B-swizzled operand stored as 32-column chunks
@@ -234,24 +235,31 @@ __device__ __forceinline__ void fz_store_row64(float* row, const float* v) {
   for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(row + 8 * j + cq) = make_float2(v[2 * j], v[2 * j + 1]);
 }
 
-// narrow / full-width row store with the optional forecast-step epilogue (P: FzParams or DecParams)
-template <class P>
+// narrow / full-width row store with the optional forecast-step epilogue (P: FzParams, DecParams or NodeParams).
+// STD (the predicted-std form of the step epilogue): the W = 2d outputs are d state deltas, then d raw stds.  Column c < d
+// takes the step epilogue, column d + c is stored as std_out[b, r, c] = softplus(y) with torch's threshold 20 and without
+// the boundary mix; prev, boundary, the new state and std_out have rows of d.
+template <bool STD = false, class P>
 __device__ __forceinline__ void fz_store_rows(const P& p, float* out, int W, long long n_rows, bool step, float (*v)[16],
                                               int b, long long r0, bool valid0, bool valid1) {
   const int cq = 2 * (threadIdx.x & 3);
+  const int Ws = STD ? W >> 1 : W;  // row pitch of the stored rows
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     if (!(i ? valid1 : valid0)) continue;
     const long long r = r0 + 8 * i;
-    const long long o = ((long long)b * n_rows + r) * W;
+    const long long o = ((long long)b * n_rows + r) * Ws;
     if (step) {
       const float mk = p.bnd ? __ldg(p.mask + r) : 0.f;
 #pragma unroll
       for (int t = 0; t < 16; ++t) {
         const int c = 8 * (t >> 1) + cq + (t & 1);
-        if (c < W) {
+        if (c < Ws) {
           const float nw = __ldg(p.prev + o + c) + (v[i][t] * __ldg(p.dstd + c) + __ldg(p.dmean + c));
           out[o + c] = p.bnd ? mk * __ldg(p.bnd + o + c) + (1.f - mk) * nw : nw;
+        } else if (STD && c < W) {
+          const float y = v[i][t];
+          p.std_out[o + c - Ws] = y > 20.f ? y : log1pf(expf(y));
         }
       }
     } else if (W == 64) {
@@ -266,6 +274,7 @@ __device__ __forceinline__ void fz_store_rows(const P& p, float* out, int W, lon
   }
 }
 
+template <bool STD>  // STD: the step epilogue's predicted-std form (fz_store_rows)
 __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_constant__ FzParams p) {
   using namespace fz;
   const Layout L = layout(p.kc1, p.mode);
@@ -385,7 +394,7 @@ __global__ void __launch_bounds__(fz::THREADS, 2) fused_mlp_kernel(const __grid_
       const float* base = p.res + (long long)b * p.res_bs;
       fz_add_rows(v, valid0 ? base + r0 * 64 : nullptr, valid1 ? base + (r0 + 8) * 64 : nullptr);
     }
-    fz_store_rows(p, p.out, p.out_w, p.n_rows, p.step, v, b, r0, valid0, valid1);
+    fz_store_rows<STD>(p, p.out, p.out_w, p.n_rows, p.step, v, b, r0, valid0, valid1);
   }
 }
 
@@ -665,8 +674,9 @@ struct DecParams {
   FzW w1r, w2e, wn1, wn2, wo1, wo2;
   const float *b2e, *gamma_e, *beta_e, *bn1, *bn2, *gamma_n, *beta_n, *bo1, *bo2;
   float eps_e, eps_n;
-  float* out;                 // (B, n_rec, D) new state
+  float* out;                 // (B, n_rec, D) new state (D / 2 wide in the STD form)
   const float *prev, *bnd, *mask, *dstd, *dmean;
+  float* std_out;             // STD form: (B, n_rec, D / 2) predicted std
 };
 
 // warp group MMA that adds to the accumulators: acc += A[rows] · Wᵀ over kc chunks
@@ -681,7 +691,8 @@ __device__ __forceinline__ void dec_gemm_add(float* acc, uint32_t a, uint32_t w,
   wgmma_wait0(acc, 32);
 }
 
-template <int DEG>  // uniform in-degree: 1, 2, 4 or 8
+// DEG: uniform in-degree 1, 2, 4 or 8; STD: the step epilogue's predicted-std form (fz_store_rows), D = 2d outputs
+template <int DEG, bool STD>
 __global__ void __launch_bounds__(dec::THREADS, 1) tc_decode_kernel(const __grid_constant__ DecParams p) {
   using namespace fz;
   extern __shared__ uint8_t smem_raw[];
@@ -756,8 +767,9 @@ __global__ void __launch_bounds__(dec::THREADS, 1) tc_decode_kernel(const __grid
       };
       load_src(0);
       {  // the epilogue's previous / boundary state rows of the item -> L2
-        const long long n = min(64LL, p.n_rec - r0) * p.D;
-        const float* spans[2] = {p.prev + ((long long)b * p.n_rec + r0) * p.D, p.bnd ? p.bnd + ((long long)b * p.n_rec + r0) * p.D : nullptr};
+        const int Ds = STD ? p.D >> 1 : p.D;  // state columns
+        const long long n = min(64LL, p.n_rec - r0) * Ds;
+        const float* spans[2] = {p.prev + ((long long)b * p.n_rec + r0) * Ds, p.bnd ? p.bnd + ((long long)b * p.n_rec + r0) * Ds : nullptr};
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           if (!spans[q]) continue;
@@ -904,7 +916,7 @@ __global__ void __launch_bounds__(dec::THREADS, 1) tc_decode_kernel(const __grid
     fz_gemm(acc, aN, sb + dec::WO2, 2);
     fz_unpack(acc, v, prm + 512);
     const long long ra = r0 + lr;
-    fz_store_rows(p, p.out, p.D, p.n_rec, true, v, b, ra, ra < p.n_rec, ra + 8 < p.n_rec);
+    fz_store_rows<STD>(p, p.out, p.D, p.n_rec, true, v, b, ra, ra < p.n_rec, ra + 8 < p.n_rec);
   }
 }
 
@@ -1328,8 +1340,10 @@ struct NodeParams {
   int out_w;
   float *out3, *out4;         // POST_PROJ: (B, n_rows, 64) each
   const float *prev, *bnd, *mask, *dstd, *dmean;  // POST_OUTMLP: the forecast-step epilogue
+  float* std_out;             // POST_OUTMLP, STD form: (B, n_rows, out_w / 2) predicted std
 };
 
+template <bool STD>  // STD: POST_OUTMLP's step epilogue in its predicted-std form (fz_store_rows)
 __global__ void __launch_bounds__(fz::THREADS, 1) tc_node_kernel(const __grid_constant__ NodeParams p) {
   using namespace fz;
   extern __shared__ uint8_t smem_raw[];
@@ -1447,7 +1461,7 @@ __global__ void __launch_bounds__(fz::THREADS, 1) tc_node_kernel(const __grid_co
       fz_store_op(sA, v, rq, wg);
       fz_gemm(acc, aA, sb + nod::W4, 2);
       fz_unpack(acc, v, prm + 320);
-      fz_store_rows(p, p.out, p.out_w, p.n_rows, true, v, b, r0, valid0, valid1);
+      fz_store_rows<STD>(p, p.out, p.out_w, p.n_rows, true, v, b, r0, valid0, valid1);
     }
   }
 }
@@ -1486,9 +1500,10 @@ static int persistent_launch(int threads, size_t smem, size_t smem_limit, long l
 }
 
 // fused_mlp_kernel: as many CTAs per SM as fit (two for the K = 64 launches); the limit covers the largest layout
+template <bool STD = false>
 static int fz_launch(const FzParams& p, const char* name, double bytes, cudaStream_t st) {
   const long long n_work = (long long)p.n_tiles * p.B + (p.mode == fz::ROWLIN ? (long long)p.n_tiles1 * p.B1 : 0);
-  return persistent_launch<fused_mlp_kernel>(fz::THREADS, fz::layout(p.kc1, p.mode).bytes, fz::layout(6, fz::EDGE).bytes, n_work,
+  return persistent_launch<fused_mlp_kernel<STD>>(fz::THREADS, fz::layout(p.kc1, p.mode).bytes, fz::layout(6, fz::EDGE).bytes, n_work,
                                              0, name, bytes, st, p);
 }
 
@@ -1518,10 +1533,11 @@ static NodeParams node_params(const NlamMlp* m, const float* src0, int64_t bs0, 
   return p;
 }
 
+template <bool STD = false>
 static int node_launch(const NodeParams& p, const char* name, double bytes, cudaStream_t st) {
   const long long n_items = p.n_tiles * p.B;
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
-  return persistent_launch<tc_node_kernel>(fz::THREADS, nod::BYTES, nod::BYTES, n_items, grid, name, bytes, st, p);
+  return persistent_launch<tc_node_kernel<STD>>(fz::THREADS, nod::BYTES, nod::BYTES, n_items, grid, name, bytes, st, p);
 }
 
 static void fz_mlp(FzParams& p, const NlamMlp* m, int k_off, int k_cols) {
@@ -1578,11 +1594,14 @@ int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamR
   const int nout = mlp->out_dim[1];
   NLAM_REQUIRE(!ep || (nout < 64 && !mlp->ln_gamma && !res), NLAM_E_UNSUPPORTED,
                "tc_rowmlp: the fused step epilogue needs a narrow output without LayerNorm / residual");
+  const bool std_form = ep && ep->std_out;
+  NLAM_REQUIRE(!std_form || nout % 2 == 0, NLAM_E_UNSUPPORTED, "tc_rowmlp: the predicted-std form needs 2·d outputs");
+  const int nst = std_form ? nout / 2 : nout;  // stored columns per row
   double bytes = 0;
   for (int s = 0; s < n_src; ++s) bytes += 4.0 * n_rows * srcs[s].dim * ((srcs[s].bstride != 0 && B > 1) ? B : 1);
   if (res) bytes += 4.0 * n_rows * 64 * ((res->bstride != 0 && B > 1) ? B : 1);
-  bytes += 4.0 * n_rows * B * nout;
-  if (ep) bytes += 4.0 * n_rows * B * nout * (ep->boundary ? 2 : 1);
+  bytes += 4.0 * n_rows * B * nst * (std_form ? 2 : 1);
+  if (ep) bytes += 4.0 * n_rows * B * nst * (ep->boundary ? 2 : 1);
   // node update: two 64-wide sources, the residual one of them
   if (res && !ep && n_src == 2 && srcs[0].dim == 64 && srcs[1].dim == 64 && node_mlp_ok(mlp)) {
     const int res_src = (srcs[0].ptr == res->ptr && srcs[0].bstride == res->bstride) ? 0 : 1;
@@ -1611,8 +1630,9 @@ int tc_rowmlp(const NlamMlp* mlp, const NlamRowSrc* srcs, int n_src, const NlamR
     p.mask = ep->mask;
     p.dstd = ep->std;
     p.dmean = ep->mean;
+    p.std_out = ep->std_out;
   }
-  return fz_launch(p, "tc_rowmlp_kernel", bytes, st);
+  return std_form ? fz_launch<true>(p, "tc_rowmlp_kernel", bytes, st) : fz_launch(p, "tc_rowmlp_kernel", bytes, st);
 }
 
 // ---- two 64 -> 64 row Linears in one launch: out0 = x0·W0ᵀ (B0 batches), out1 = x1·W1ᵀ + b1 (B1 batches); W0, W1 are
@@ -1805,6 +1825,7 @@ bool tc_node_out_supported(const NlamMlp* node_mlp, const NlamMlp* out_mlp, cons
   if (n_rows < 1 || n_rows >= (1LL << 31) - 256 || !node_mlp_ok(node_mlp)) return false;
   if (!mlp_shape_ok(out_mlp, &no2) || no2 >= 64 || out_mlp->in_dim != 64 || out_mlp->ln_gamma) return false;
   if (!(aligned16(rec) && aligned16(aggr) && rec_bs % 4 == 0 && out)) return false;
+  if (ep && ep->std_out && no2 % 2) return false;  // the predicted-std form: 2·d outputs
   return ep && ep->prev && ep->std && ep->mean && (!ep->boundary || ep->mask);
 }
 
@@ -1825,8 +1846,11 @@ int tc_node_out(const NlamMlp* node_mlp, const NlamMlp* out_mlp, const float* re
   p.mask = ep->mask;
   p.dstd = ep->std;
   p.dmean = ep->mean;
-  const double bytes = 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + 3.0 * D * B);
-  return node_launch(p, "tc_node_out_kernel", bytes, st);
+  p.std_out = ep->std_out;
+  // previous / new (/ boundary) state and the std: d = D (D / 2 in the predicted-std form) columns each
+  const bool std_form = ep->std_out != nullptr;
+  const double bytes = 4.0 * n_rows * (64.0 * (((rec_bs != 0 && B > 1) ? B : 1) + B) + (std_form ? 4.0 * (D / 2) : 3.0 * D) * B);
+  return std_form ? node_launch<true>(p, "tc_node_out_kernel", bytes, st) : node_launch(p, "tc_node_out_kernel", bytes, st);
 }
 
 // ---- mesh -> grid decoder: edge projections (tc_rowlinear_kernel) + tc_decode_kernel
@@ -1847,6 +1871,7 @@ bool tc_decode_supported(const NlamGraph* g, const NlamMlp* edge_mlp, const Nlam
   if (!(edge_bs == 0 || B == 1)) return false;  // edge features shared by the batch: P_e is computed once
   if (!(aligned16(send) && aligned16(rec) && aligned16(edge) && send_bs % 4 == 0 && rec_bs % 4 == 0 && out)) return false;
   if (B > 1 && send_bs != 0 && send_bs < g->n_send * 64) return false;
+  if (ep && ep->std_out && no % 2) return false;  // the predicted-std form: 2·d outputs
   return ep && ep->prev && ep->std && ep->mean && (!ep->boundary || ep->mask);
 }
 
@@ -1903,17 +1928,23 @@ int tc_decode(const NlamGraph* g, const NlamMlp* edge_mlp, const NlamMlp* node_m
   p.mask = ep->mask;
   p.dstd = ep->std;
   p.dmean = ep->mean;
+  p.std_out = ep->std_out;
+  const bool std_form = ep->std_out != nullptr;
   const long long n_items = p.n_blocks * B;
   const int grid = (int)std::min<long long>((n_items + 1) / 2, num_sms());  // one CTA per SM, two items at a time
-  // algorithmic bytes: receivers, P_s, P_e and the sender indices once, previous / new (/ boundary) state, weights
-  const int D = p.D, Br = (rec_bs != 0 && B > 1) ? B : 1;
+  // algorithmic bytes: receivers, P_s, P_e and the sender indices once, previous / new (/ boundary) state and the std
+  // (Ds columns each), weights
+  const int D = p.D, Ds = std_form ? D / 2 : D, Br = (rec_bs != 0 && B > 1) ? B : 1;
   const double bytes = 256.0 * ((double)g->n_rec * Br + (double)g->n_send * Bs + (double)g->n_edges) + 4.0 * g->n_edges +
-                       4.0 * (double)g->n_rec * D * B * (ep->boundary ? 3 : 2) + (ep->boundary ? 4.0 * g->n_rec : 0.0) +
-                       4.0 * (7 * 64 * 64 + 64 * D + 9 * 64);
-  const auto launch = p.d == 1   ? persistent_launch<tc_decode_kernel<1>, DecParams>
-                      : p.d == 2 ? persistent_launch<tc_decode_kernel<2>, DecParams>
-                      : p.d == 4 ? persistent_launch<tc_decode_kernel<4>, DecParams>
-                                 : persistent_launch<tc_decode_kernel<8>, DecParams>;
+                       4.0 * (double)g->n_rec * Ds * B * ((ep->boundary ? 3 : 2) + (std_form ? 1 : 0)) +
+                       (ep->boundary ? 4.0 * g->n_rec : 0.0) + 4.0 * (7 * 64 * 64 + 64 * D + 9 * 64);
+  using Launch = int (*)(int, size_t, size_t, long long, int, const char*, double, cudaStream_t, const DecParams&);
+  static const Launch launches[2][4] = {
+      {persistent_launch<tc_decode_kernel<1, false>, DecParams>, persistent_launch<tc_decode_kernel<2, false>, DecParams>,
+       persistent_launch<tc_decode_kernel<4, false>, DecParams>, persistent_launch<tc_decode_kernel<8, false>, DecParams>},
+      {persistent_launch<tc_decode_kernel<1, true>, DecParams>, persistent_launch<tc_decode_kernel<2, true>, DecParams>,
+       persistent_launch<tc_decode_kernel<4, true>, DecParams>, persistent_launch<tc_decode_kernel<8, true>, DecParams>}};
+  const Launch launch = launches[std_form][p.d == 1 ? 0 : p.d == 2 ? 1 : p.d == 4 ? 2 : 3];
   return launch(dec::THREADS, dec::BYTES, dec::BYTES, n_items, grid, "tc_decode_kernel", bytes, st, p);
 }
 

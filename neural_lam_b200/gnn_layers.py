@@ -377,16 +377,17 @@ class InteractionNet(nn.Module):
 
     @torch.no_grad()
     def decode_step(self, send_rep, rec_rep, edge_rep, out_seq, prev, boundary, bmask, diff_std, diff_mean, out_flags=0,
-                    out=None):
+                    out=None, std_out=None):
         """Inference-only: this layer (the mesh->grid decoder) chained with ``out_seq`` and the forecast-step epilogue in two
         launches (``ops.decode_step``); neither the aggregate nor the updated receiver rows go to HBM.  Returns the new state,
-        or None when the layer / graph / call shape has no such path (the caller then runs ``aggregate_only``)."""
+        or None when the layer / graph / call shape has no such path (the caller then runs ``aggregate_only``).  ``std_out``:
+        the predicted-std form of ``ops.decode_step``."""
         if not self._edge_stage_separable() or (out_flags & _lib.MATH_FP32):
             return None
         self._check_inputs(send_rep, rec_rep, edge_rep)
         _, (s3, r3, e3) = self._batchify(send_rep, rec_rep, edge_rep)
         return ops.decode_step(self._graph(r3.device), self.edge_mlp, self.aggr_mlp, out_seq, s3, r3, e3, prev, boundary, bmask,
-                               diff_std, diff_mean, flags=self._flags() | out_flags, out=out)
+                               diff_std, diff_mean, flags=self._flags() | out_flags, out=out, std_out=std_out)
 
     @torch.no_grad()
     def encode_step(self, embedder, grid_mlp, grid_inputs, rec_rep, edge_rep, want_grid_emb=False, second=None):

@@ -259,18 +259,37 @@ class BaseGraphModel(StepPredictor):
         rescaled = pred_delta_mean * self.diff_std + self.diff_mean
         return self.get_clamped_new_state(rescaled, prev_state), pred_std
 
+    def _check_std_out(self, std_out, prev_state):
+        """``std_out`` of ``forward_with_boundary``: required, a dense (B, G, d) float32 tensor on prev_state's device, for a
+        model that predicts its std; refused for one that does not."""
+        if not self.output_std:
+            if std_out is not None:
+                raise ValueError(f"std_out given, but this {type(self).__name__} does not predict a std (output_std=False)")
+            return
+        if std_out is None:
+            raise ValueError(f"this {type(self).__name__} predicts a std (output_std=True): pass std_out, a (B, G, d) tensor "
+                             "on the device")
+        if (tuple(std_out.shape) != tuple(prev_state.shape) or std_out.device != prev_state.device
+                or std_out.dtype != torch.float32 or not std_out.is_contiguous()):
+            raise ValueError(f"std_out: expected a contiguous float32 tensor of shape {tuple(prev_state.shape)} on "
+                             f"{prev_state.device}, got {tuple(std_out.shape)} {std_out.dtype} on {std_out.device}")
+
     @torch.no_grad()
-    def forward_with_boundary(self, prev_state, prev_prev_state, forcing, boundary_state, boundary_mask, out=None):
+    def forward_with_boundary(self, prev_state, prev_prev_state, forcing, boundary_state, boundary_mask, out=None,
+                              std_out=None):
         """Inference step with the ARForecaster boundary mix (autoregressive.py:128-131) fused
-        into the step epilogue kernel.  ``out``: optional preallocated (B,G,d) tensor for the new state."""
-        assert not self.output_std
+        into the step epilogue kernel.  ``out``: optional preallocated (B,G,d) tensor for the new state.
+        ``std_out``: for a model that predicts its std (and only for one), the (B,G,d) device tensor that
+        receives the step's std (softplus of the second half of output_map, not boundary-mixed).  Returns
+        the new state."""
+        self._check_std_out(std_out, prev_state)
         B = prev_state.shape[0]
         st, mesh_rep, grid_rep = self._encode(prev_state, prev_prev_state, forcing)
         mesh_rep = self.process_step(mesh_rep, st)
         return self._decode(self.m2g_gnn, self.output_map, mesh_rep, grid_rep, self.expand_to_batch(st["m2g_emb"], B), prev_state,
-                            boundary_state, boundary_mask, out)[0]
+                            boundary_state, boundary_mask, out, std_out)[0]
 
-    def _decode(self, m2g, out_map, mesh_rep, grid_rep, m2g_emb, prev_state, boundary, bmask, out=None):
+    def _decode(self, m2g, out_map, mesh_rep, grid_rep, m2g_emb, prev_state, boundary, bmask, out=None, std_out=None):
         """The no-grad decoder: the mesh -> grid layer ``m2g``, the output MLP ``out_map``, the rescale and (clamped) residual
         update (graph/base.py:322-342, step_predictors/base.py:366-396) and the boundary mix (autoregressive.py:128-131;
         ``boundary`` None: none) -> (new_state, pred_std|None).  The first of these that covers the call runs:
@@ -278,26 +297,29 @@ class BaseGraphModel(StepPredictor):
           2. ``m2g.aggregate_only``, then the node update, ``out_map`` and the step epilogue in one launch
              (``ops.node_update_step``): the updated grid representation never goes to HBM;
           3. the m2g layer, then ``out_map`` and the step epilogue in one launch (``ops.rowmlp_step``);
-          4. the m2g layer, ``out_map`` and ``ops.step_epilogue``: the one rung for clamped outputs and a predicted std."""
+          4. the m2g layer, ``out_map`` and ``ops.step_epilogue``: the one rung for clamped outputs, and for a predicted std
+             without ``std_out``.
+        ``std_out`` (a model that predicts its std): rungs 1-3 run their predicted-std forms, which write the std there, and
+        rung 4 writes it there with torch ops; pred_std is then ``std_out``."""
         clamp = (self._clamp_kind, self._clamp_lo, self._clamp_up) if self.clamps_output else None
-        if clamp is None and not self.output_std:
+        if clamp is None and (not self.output_std or std_out is not None):
             fused = m2g.decode_step(mesh_rep, grid_rep, m2g_emb, out_map, prev_state, boundary, bmask, self.diff_std,
-                                    self.diff_mean, out_flags=out_map.nlam_flags, out=out)
+                                    self.diff_mean, out_flags=out_map.nlam_flags, out=out, std_out=std_out)
             if fused is not None:
-                return fused, None
+                return fused, std_out
             aggr = m2g.aggregate_only(mesh_rep, grid_rep, m2g_emb)
             if aggr is not None:
                 fused = ops.node_update_step(m2g.aggr_mlp, out_map, grid_rep, aggr, prev_state, boundary, bmask, self.diff_std,
-                                             self.diff_mean, flags=out_map.nlam_flags, out=out)
+                                             self.diff_mean, flags=out_map.nlam_flags, out=out, std_out=std_out)
                 if fused is not None:
-                    return fused, None
+                    return fused, std_out
                 grid_rep = m2g._kernel_node_update(grid_rep, aggr)
             else:
                 grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
             fused = ops.rowmlp_step(out_map, grid_rep, prev_state, boundary, bmask, self.diff_std, self.diff_mean,
-                                    flags=out_map.nlam_flags, out=out)
+                                    flags=out_map.nlam_flags, out=out, std_out=std_out)
             if fused is not None:
-                return fused, None
+                return fused, std_out
         else:
             grid_rep = m2g(mesh_rep, grid_rep, m2g_emb)
         net_output = out_map(grid_rep)
@@ -305,6 +327,8 @@ class BaseGraphModel(StepPredictor):
         if self.output_std:
             net_output, std_raw = net_output.chunk(2, dim=-1)
             pred_std = torch.nn.functional.softplus(std_raw)
+            if std_out is not None:
+                pred_std = std_out.copy_(pred_std)
         return ops.step_epilogue(net_output, prev_state, boundary, bmask, self.diff_std, self.diff_mean, out=out,
                                  clamp=clamp), pred_std
 
@@ -631,13 +655,14 @@ class BaseGraphEFM(BaseGraphModel):
 
     @torch.no_grad()
     def forward_with_boundary(self, prev_state, prev_prev_state, forcing, boundary_state, boundary_mask, latent_noise=None,
-                              out=None):
+                              out=None, std_out=None):
         """Inference step with the ARForecaster boundary mix fused into the step epilogue.  ``out``: optional preallocated
-        (B,G,d) tensor for the new state."""
-        assert not self.output_std
-        return self._step(prev_state, prev_prev_state, forcing, latent_noise, boundary_state, boundary_mask, out)[0]
+        (B,G,d) tensor for the new state; ``std_out``: the (B,G,d) tensor for the predicted std, required for a model that
+        predicts it and refused otherwise (``BaseGraphModel.forward_with_boundary``).  Returns the new state."""
+        self._check_std_out(std_out, prev_state)
+        return self._step(prev_state, prev_prev_state, forcing, latent_noise, boundary_state, boundary_mask, out, std_out)[0]
 
-    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
+    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out, std_out=None):
         raise NotImplementedError
 
     def _sample_latent(self, mesh_rep, grid_emb, eps):
@@ -713,7 +738,7 @@ class GraphEFMMultiScale(BaseGraphEFM):
         return {"mesh": ge["mesh"], "m2m": ge["m2m"]}
 
     @torch.no_grad()
-    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
+    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out, std_out=None):
         """The no-grad step: (1) grid embedder, decoder grid MLP and the prior g2m's projections in one launch, (2) prior g2m,
         (3) prior m2m stack, (4) prior parameters + sample + latent embedding in one launch, (5) decoder g2m, (6) decoder
         m2m stack, (7) m2g + param_map + step epilogue.  Each fused launch falls back to its composition where the library
@@ -729,7 +754,7 @@ class GraphEFMMultiScale(BaseGraphEFM):
         mesh_rep = prior.process_mesh(prior_reps[0], ge["m2m"]) if learned else None
         latent_emb = self._sample_latent(mesh_rep, grid_emb, eps)
         mesh_rep = dec.mesh_step(grid_emb, latent_emb, ge)
-        return self._decode(dec.m2g_gnn, dec.param_map, mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+        return self._decode(dec.m2g_gnn, dec.param_map, mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out, std_out)
 
 
 class GraphEFM(BaseGraphEFM):
@@ -812,7 +837,7 @@ class GraphEFM(BaseGraphEFM):
         return {k: ge[k] for k in ("mesh", "mesh_up", "mesh_down", "m2m")}
 
     @torch.no_grad()
-    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out):
+    def _step(self, prev_state, prev_prev_state, forcing, latent_noise, boundary, bmask, out, std_out=None):
         """The no-grad step: (1) grid embedder, decoder grid MLP and the projections of both g2m layers (the prior's and the
         decoder's: both have the static level-0 embedding as receivers) in one launch, then both g2m layers on their
         projections, (2) the prior's sweep up the hierarchy, (3) prior parameters + sample + latent embedding in one launch,
@@ -831,7 +856,7 @@ class GraphEFM(BaseGraphEFM):
         # the constant prior reads only the batch size and device of its input: res_grid stands in for the grid embedding
         latent_emb = self._sample_latent(prior_rep, res_grid, eps)
         mesh_rep = dec.mesh_step(reps[-1], latent_emb, ge)
-        return self._decode(dec.m2g_gnn, dec.param_map, mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out)
+        return self._decode(dec.m2g_gnn, dec.param_map, mesh_rep, res_grid, ge["m2g"], prev_state, boundary, bmask, out, std_out)
 
 
 MODELS = {"graph_lam": GraphLAM, "hi_lam": HiLAM, "hi_lam_parallel": HiLAMParallel}
@@ -938,7 +963,8 @@ class ARForecaster(nn.Module):
         The states live in a ring of three buffers — step k reads prev_prev = state[k%3], prev = state[(k+1)%3] and
         writes the new state into state[(k+2)%3] — so the autoregressive feedback costs no copies; the three
         rotations are three graphs sharing one memory pool.  Returns the dict of static buffers
-        (``forcing``, ``boundary``, ``state``)."""
+        (``forcing``, ``boundary``, ``state`` and, for a predictor that predicts its std, ``std``: the std of the step
+        replayed last)."""
         p = self.predictor
         bufs = self._step_buffers(batch_size)
         p.static_embeddings()  # materialise the weight-only embeddings outside the graph
@@ -952,8 +978,8 @@ class ARForecaster(nn.Module):
         return bufs
 
     def _step_buffers(self, batch_size):
-        """The static buffers of a captured step on ``batch_size`` rows: ``forcing``, ``boundary``, the ``state`` ring and,
-        for a sampling predictor, ``latent_noise``."""
+        """The static buffers of a captured step on ``batch_size`` rows: ``forcing``, ``boundary``, the ``state`` ring, for a
+        sampling predictor ``latent_noise`` and for a predictor that predicts its std ``std``."""
         p = self.predictor
         dev = self.boundary_mask.device
         G, d, f = p.num_grid_nodes, p.num_state_vars, p.grid_input_dim - 2 * p.num_state_vars - p.grid_static_features.shape[1]
@@ -963,6 +989,8 @@ class ARForecaster(nn.Module):
             # a predictor that samples: every captured step first refills this buffer from the default generator of the
             # device, so each replay draws fresh noise and torch.cuda.manual_seed makes a sequence of replays reproducible
             bufs["latent_noise"] = torch.zeros(batch_size, p.latent_spatial_dim, p.latent_dim, device=dev)
+        if p.predicts_std:
+            bufs["std"] = torch.zeros(batch_size, G, d, device=dev)
         return bufs
 
     def _capture_ring(self, step):
@@ -997,12 +1025,13 @@ class ARForecaster(nn.Module):
     def _one_step(self, bufs, k):
         st = bufs["state"]
         noise = bufs.get("latent_noise")
+        std = bufs["std"] if self.predicts_std else None  # (the ensemble's buffers use "std" for the member spread)
         if noise is None:
             return self.predictor.forward_with_boundary(st[(k + 1) % 3], st[k % 3], bufs["forcing"], bufs["boundary"],
-                                                        self.boundary_mask, out=st[(k + 2) % 3])
+                                                        self.boundary_mask, out=st[(k + 2) % 3], std_out=std)
         noise.normal_()
         return self.predictor.forward_with_boundary(st[(k + 1) % 3], st[k % 3], bufs["forcing"], bufs["boundary"],
-                                                    self.boundary_mask, latent_noise=noise, out=st[(k + 2) % 3])
+                                                    self.boundary_mask, latent_noise=noise, out=st[(k + 2) % 3], std_out=std)
 
     def set_state(self, prev_prev_state, prev_state):
         """Load the two initial states into the captured step's state ring."""
@@ -1020,10 +1049,24 @@ class ARForecaster(nn.Module):
         self._phase = (k + 1) % 3
         return bufs["state"][(k + 2) % 3]
 
+    def _check_std_out(self, std_out, shape, on_device):
+        """``std_out`` of a rollout: only for a predictor that predicts its std, of ``shape`` (B, T, G, d), float32, on the
+        device (``on_device``) or on the host."""
+        if std_out is None:
+            return
+        if not self.predicts_std:
+            raise ValueError(f"std_out given, but {type(self.predictor).__name__} does not predict a std (output_std=False)")
+        where = "device" if on_device else "host"
+        if tuple(std_out.shape) != tuple(shape) or std_out.dtype != torch.float32 or std_out.is_cuda != on_device:
+            raise ValueError(f"std_out: expected a float32 {where} tensor of shape {tuple(shape)}, got {tuple(std_out.shape)} "
+                             f"{std_out.dtype} on {std_out.device}")
+
     @torch.no_grad()
-    def rollout_graphed(self, init_states, forcing_features, boundary_states):
-        """Same result as ``forward`` (no std), replaying the captured step graphs."""
+    def rollout_graphed(self, init_states, forcing_features, boundary_states, std_out=None):
+        """Same prediction as ``forward``, replaying the captured step graphs; returns it (B,T,G,d).  ``std_out``: a (B,T,G,d)
+        device tensor that receives each step's std, for a predictor that predicts it."""
         B, T = forcing_features.shape[0], forcing_features.shape[1]
+        self._check_std_out(std_out, (B, T) + tuple(init_states.shape[2:]), True)
         self._ensure_captured(B)
         _, _, bufs = self._graph
         out = torch.empty(B, T, *init_states.shape[2:], device=init_states.device)
@@ -1032,6 +1075,8 @@ class ARForecaster(nn.Module):
             bufs["forcing"].copy_(forcing_features[:, i])
             bufs["boundary"].copy_(boundary_states[:, i])
             out[:, i].copy_(self.replay_step())
+            if std_out is not None:
+                std_out[:, i].copy_(bufs["std"])
         return out
 
     # ---- ensemble forecasts of a sampling predictor: K members per initial condition, reduced on the device ----------
@@ -1081,6 +1126,9 @@ class ARForecaster(nn.Module):
         p = self.predictor
         if not getattr(p, "samples_latent", False):
             raise ValueError(f"rollout_ensemble needs a predictor that samples its latent (Graph-EFM), got {type(p).__name__}")
+        if p.predicts_std:
+            raise ValueError("rollout_ensemble: the ensemble statistics of a predictor that predicts its std "
+                             "(output_std=True) are not supported")
         if isinstance(members, bool) or not isinstance(members, int) or not 2 <= members <= ensemble.MAX_MEMBERS:
             raise ValueError(f"rollout_ensemble: members must be an int in 2 .. {ensemble.MAX_MEMBERS}, got {members!r}")
         G, d = p.num_grid_nodes, p.num_state_vars
@@ -1200,22 +1248,24 @@ class ARForecaster(nn.Module):
     @torch.no_grad()
     def host_io_bytes_per_step(self, B):
         """(host->device, device->host) bytes ``rollout_from_host`` moves per AR step of B forecasts: the forcing, the rows of
-        the boundary state the boundary mask selects, and the prediction."""
+        the boundary state the boundary mask selects, and the prediction (and its std, for a predictor that predicts it)."""
         self._ensure_captured(B)
         _, _, bufs = self._graph
         G, d_state = bufs["boundary"].shape[1], bufs["boundary"].shape[2]
         blocks = _boundary_blocks(self.boundary_mask)
         bnd_rows = G if blocks is None else sum(rlen * count for _, rlen, _, count in blocks)
-        return B * (G * bufs["forcing"].shape[2] + bnd_rows * d_state) * 4, B * G * d_state * 4
+        return B * (G * bufs["forcing"].shape[2] + bnd_rows * d_state) * 4, B * G * d_state * 4 * (2 if self.predicts_std else 1)
 
-    def rollout_from_host(self, init_states, forcing_features, boundary_states, out=None):
+    def rollout_from_host(self, init_states, forcing_features, boundary_states, out=None, std_out=None):
         """Inference rollout with HOST tensors (ideally pinned).  Every AR step copies that step's
         forcing + boundary states host->device, replays the captured step graph and copies the
         predicted state device->host.  The PCIe transfers run on their own streams, double
         buffered, so that H2D of step i+1 and D2H of step i-1 overlap the kernels of step i;
         nothing synchronises with the host until the end.  Shapes as in ``forward``; returns the
-        (B,T,G,d) prediction on the host (``out`` if given)."""
+        (B,T,G,d) prediction on the host (``out`` if given).  ``std_out``: a (B,T,G,d) host tensor
+        that receives each step's std (for a predictor that predicts it), copied as the prediction is."""
         B, T = forcing_features.shape[0], forcing_features.shape[1]
+        self._check_std_out(std_out, (B, T) + tuple(init_states.shape[2:]), False)
         dev = self.boundary_mask.device
         self._ensure_captured(B)
         _, _, bufs = self._graph
@@ -1229,6 +1279,7 @@ class ARForecaster(nn.Module):
                 # zero mask in the step epilogue)
                 "bnd": [torch.zeros_like(bufs["boundary"]) for _ in range(2)],
                 "out": [torch.empty_like(bufs["boundary"]) for _ in range(2)],
+                "std": [torch.empty_like(bufs["std"]) for _ in range(2)] if self.predicts_std else None,
                 "bnd_blocks": _boundary_blocks(self.boundary_mask),
             }
         io = self._io
@@ -1253,7 +1304,9 @@ class ARForecaster(nn.Module):
                     and t.stride(2) == t.shape[3] and t.stride(1) == t.shape[2] * t.shape[3]
                     and t.stride(0) % (t.shape[2] * t.shape[3]) == 0)
 
-        dense = all(sliceable(t) for t in (forcing_features, boundary_states, out))
+        # (device staging buffers, host tensor) of every per-step device -> host copy
+        d2h = [(io["out"], out)] + ([(io["std"], std_out)] if std_out is not None else [])
+        dense = all(sliceable(t) for t in (forcing_features, boundary_states) + tuple(h for _, h in d2h))
 
         def copy_boundary(dev_t, host_t, i, stream):
             """only the rows the boundary mask selects (new = mask*boundary + (1-mask)*prediction never reads the others):
@@ -1305,14 +1358,17 @@ class ARForecaster(nn.Module):
             if i >= 2:
                 main.wait_event(out_free[k])
             io["out"][k].copy_(new_state)
+            if std_out is not None:
+                io["std"][k].copy_(bufs["std"])
             out_ready[k].record(main)
             with torch.cuda.stream(s_out):
                 s_out.wait_event(out_ready[k])
-                if dense:
-                    copy_step(io["out"][k], out, i, s_out, False)
-                else:
-                    for b in range(B):
-                        out[b, i].copy_(io["out"][k][b], non_blocking=True)
+                for stage, host in d2h:
+                    if dense:
+                        copy_step(stage[k], host, i, s_out, False)
+                    else:
+                        for b in range(B):
+                            host[b, i].copy_(stage[k][b], non_blocking=True)
                 out_free[k].record(s_out)
         main.wait_stream(s_out)
         main.wait_stream(s_in)

@@ -133,6 +133,15 @@ def _ptr(t):
     return t.data_ptr() if t is not None else None
 
 
+def _std_io(std_out, prev, n_out):
+    """The predicted-std form of a fused step: ``std_out`` (a dense float32 device tensor of prev's shape (B, G, d)) and
+    the MLP's output count ``n_out`` (2·d) -> whether the fused kernels can take the call (False: the widths disagree)."""
+    if tuple(std_out.shape) != tuple(prev.shape) or not std_out.is_contiguous():
+        raise ValueError(f"std_out: expected a contiguous tensor of shape {tuple(prev.shape)}, got {tuple(std_out.shape)}")
+    _require_cuda(std_out)
+    return n_out == 2 * prev.shape[-1]
+
+
 def rowmlp(seq, sources, res=None, flags=0, idx=None, res_idx=None, row_range=None):
     """``out[r] = (res[res_idx[r]] or 0) + seq(cat_s sources_s[idx_s[r]])`` for rows r in
     ``row_range`` (default all) with the row-MLP kernels (``nlam_rowmlp_fwd``).
@@ -392,10 +401,12 @@ def step_epilogue(net_out, prev, boundary, bmask, diff_std, diff_mean, out=None,
     return out
 
 
-def rowmlp_step(seq, x, prev, boundary, bmask, diff_std, diff_mean, flags=0, out=None):
+def rowmlp_step(seq, x, prev, boundary, bmask, diff_std, diff_mean, flags=0, out=None, std_out=None):
     """``bmask*boundary + (1-bmask)*(prev + (seq(x)*diff_std + diff_mean))`` in ONE launch
     (``nlam_rowmlp_step_fwd``: output_map + the forecast-step epilogue); returns None when the
-    library does not fuse this shape / math mode (the caller then runs the two kernels)."""
+    library does not fuse this shape / math mode (the caller then runs the two kernels).
+    ``std_out`` (prev's shape (B, G, d)): ``seq`` has 2·d outputs, the first d take the epilogue and
+    ``std_out = softplus(the last d)`` (``nlam_rowmlp_step_std_fwd``)."""
     L = _lib.lib()
     if flags & _lib.MATH_FP32:
         return None
@@ -403,23 +414,30 @@ def rowmlp_step(seq, x, prev, boundary, bmask, diff_std, diff_mean, flags=0, out
     _require_cuda(xr, prev, diff_std, diff_mean, boundary, bmask)
     mlp = mlp_struct(seq)
     G = xr.shape[-2]
-    if prev.shape != (B, G, mlp.out_dim[mlp.n_linear - 1]):
+    n_out = mlp.out_dim[mlp.n_linear - 1]
+    if std_out is not None:
+        if prev.shape[:2] != (B, G) or not _std_io(std_out, prev, n_out):
+            return None
+    elif prev.shape != (B, G, n_out):
         return None
     prev, boundary, bmask, out = _step_io(prev, boundary, bmask, out)
     with torch.cuda.device(xr.device):
-        rc = L.nlam_rowmlp_step_fwd(ctypes.byref(mlp), _row_srcs([(xr, B, bs)]), 1, prev.data_ptr(), _ptr(boundary), _ptr(bmask),
-                                    diff_std.data_ptr(), diff_mean.data_ptr(), out.data_ptr(), G, B, flags,
-                                    _stream_ptr(xr.device))
+        args = (ctypes.byref(mlp), _row_srcs([(xr, B, bs)]), 1, prev.data_ptr(), _ptr(boundary), _ptr(bmask), diff_std.data_ptr(),
+                diff_mean.data_ptr(), out.data_ptr())
+        tail = (G, B, flags, _stream_ptr(xr.device))
+        rc = (L.nlam_rowmlp_step_fwd(*args, *tail) if std_out is None
+              else L.nlam_rowmlp_step_std_fwd(*args, std_out.data_ptr(), *tail))
     if rc == _lib.E_UNSUPPORTED:
         return None
     _lib.check(rc)
     return out
 
 
-def node_update_step(node_seq, out_seq, rec, aggr, prev, boundary, bmask, diff_std, diff_mean, flags=0, out=None):
+def node_update_step(node_seq, out_seq, rec, aggr, prev, boundary, bmask, diff_std, diff_mean, flags=0, out=None, std_out=None):
     """``bmask*boundary + (1-bmask)*(prev + out_seq(rec + node_seq([rec | aggr]))*diff_std + diff_mean)`` in ONE launch
     (``nlam_node_update_step_fwd``: node update of the mesh->grid layer + output_map + forecast-step epilogue; the updated
-    grid representation never goes to HBM).  Returns None when the library does not fuse this shape / math mode."""
+    grid representation never goes to HBM).  Returns None when the library does not fuse this shape / math mode.
+    ``std_out``: the predicted-std form as in ``rowmlp_step`` (``nlam_node_update_step_std_fwd``)."""
     L = _lib.lib()
     if flags & _lib.MATH_FP32:
         return None
@@ -430,14 +448,20 @@ def node_update_step(node_seq, out_seq, rec, aggr, prev, boundary, bmask, diff_s
     D = om.out_dim[om.n_linear - 1]
     G = rr.shape[-2]
     Bt = max(B, Ba)
+    if std_out is not None:
+        if not _std_io(std_out, prev, D):
+            return None
+        D //= 2
     if (rr.shape[-1] != 64 or ar.shape[-1] != 64 or ar.shape[-2] != G or prev.shape != (Bt, G, D) or Ba != Bt
             or (Bt > 1 and abs_ != G * 64) or B not in (1, Bt)):
         return None
     prev, boundary, bmask, out = _step_io(prev, boundary, bmask, out)
     with torch.cuda.device(rr.device):
-        rc = L.nlam_node_update_step_fwd(ctypes.byref(nm), ctypes.byref(om), rr.data_ptr(), rbs if B > 1 else 0, ar.data_ptr(),
-                                         prev.data_ptr(), _ptr(boundary), _ptr(bmask), diff_std.data_ptr(),
-                                         diff_mean.data_ptr(), out.data_ptr(), G, Bt, flags, _stream_ptr(rr.device))
+        args = (ctypes.byref(nm), ctypes.byref(om), rr.data_ptr(), rbs if B > 1 else 0, ar.data_ptr(), prev.data_ptr(),
+                _ptr(boundary), _ptr(bmask), diff_std.data_ptr(), diff_mean.data_ptr(), out.data_ptr())
+        tail = (G, Bt, flags, _stream_ptr(rr.device))
+        rc = (L.nlam_node_update_step_fwd(*args, *tail) if std_out is None
+              else L.nlam_node_update_step_std_fwd(*args, std_out.data_ptr(), *tail))
     if rc == _lib.E_UNSUPPORTED:
         return None
     _lib.check(rc)
@@ -445,12 +469,13 @@ def node_update_step(node_seq, out_seq, rec, aggr, prev, boundary, bmask, diff_s
 
 
 def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, boundary, bmask, diff_std, diff_mean, flags=0,
-                out=None):
+                out=None, std_out=None):
     """The whole mesh->grid decoder of a forecast step in two launches (``nlam_decode_step_fwd``): the edge projections,
     then one kernel for the messages, the per-receiver aggregation, the node update ``rec + node_seq([rec | aggr])``,
     ``out_seq`` and the forecast-step epilogue ``bmask*boundary + (1-bmask)*(prev + y*diff_std + diff_mean)``.
     ``edge_csr``: edge features in CSR edge order, shared by the batch.  Returns None when the library does not fuse this
-    graph / shape / math mode (the caller then runs ``inet_fwd(edge_only=True)`` + ``node_update_step``)."""
+    graph / shape / math mode (the caller then runs ``inet_fwd(edge_only=True)`` + ``node_update_step``).  ``std_out``: the
+    predicted-std form as in ``rowmlp_step`` (``nlam_decode_step_std_fwd``)."""
     L = _lib.lib()
     if flags & _lib.MATH_FP32:
         return None
@@ -462,6 +487,10 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
     em, nm, om = mlp_struct(edge_seq), mlp_struct(node_seq), mlp_struct(out_seq)
     D = om.out_dim[om.n_linear - 1]
     G = r.shape[-2]
+    if std_out is not None:
+        if not _std_io(std_out, prev, D):
+            return None
+        D //= 2
     if (any(b not in (1, B) for b in (Bs, Br, Be)) or (Be > 1 and ebs != 0) or r.shape[-1] != 64 or s.shape[-1] != 64
             or e.shape[-1] != 64 or G != graph.n_rec or s.shape[-2] < graph.n_send or e.shape[-2] != graph.n_edges
             or prev.shape != (B, G, D) or r.device != graph.device):
@@ -471,10 +500,12 @@ def decode_step(graph, edge_seq, node_seq, out_seq, send, rec, edge_csr, prev, b
     ws_bytes = L.nlam_decode_workspace_bytes(graph.handle, B)
     ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
     with torch.cuda.device(dev):
-        rc = L.nlam_decode_step_fwd(graph.handle, ctypes.byref(em), ctypes.byref(nm), ctypes.byref(om),
-                                    s.data_ptr(), sbs if Bs > 1 else 0, r.data_ptr(), rbs if Br > 1 else 0, e.data_ptr(),
-                                    ebs if Be > 1 else 0, prev.data_ptr(), _ptr(boundary), _ptr(bmask), diff_std.data_ptr(),
-                                    diff_mean.data_ptr(), out.data_ptr(), B, flags, ws.data_ptr(), ws_bytes, _stream_ptr(dev))
+        args = (graph.handle, ctypes.byref(em), ctypes.byref(nm), ctypes.byref(om), s.data_ptr(), sbs if Bs > 1 else 0,
+                r.data_ptr(), rbs if Br > 1 else 0, e.data_ptr(), ebs if Be > 1 else 0, prev.data_ptr(), _ptr(boundary),
+                _ptr(bmask), diff_std.data_ptr(), diff_mean.data_ptr(), out.data_ptr())
+        tail = (B, flags, ws.data_ptr(), ws_bytes, _stream_ptr(dev))
+        rc = (L.nlam_decode_step_fwd(*args, *tail) if std_out is None
+              else L.nlam_decode_step_std_fwd(*args, std_out.data_ptr(), *tail))
     if rc == _lib.E_UNSUPPORTED:
         return None
     _lib.check(rc)
