@@ -49,6 +49,32 @@ struct ProfScope {
 
 constexpr int kTileEdges = 128;  // rows of one tensor-core edge tile
 
+// LayerNorm statistics of one row held by the 4 threads of a quad (lanes 4q .. 4q + 3, as in a wgmma accumulator
+// fragment), each with n of the row's 4n values in v.  The mean comes first, summed over the values shifted by the row's
+// first value k (quad lane 0's v[0]); then the mean square deviation from it over the same registers.  The one-pass
+// E[x²] − μ² cancels catastrophically once |μ| is large against the row's spread (|μ| / σ = 1 000 put x̂ off by about 1);
+// this form keeps x̂ at the resolution of the fp32 inputs, and the shift makes μ of a constant row exactly its value, so
+// its v − μ is exactly 0.  Every lane of the quad returns the same μ and rstd = 1 / sqrt(var + eps).
+template <int n>
+__device__ __forceinline__ void quad_row_stats(const float* v, float eps, float& mu, float& rstd) {
+  const float k = __shfl_sync(0xffffffffu, v[0], 0, 4);
+  float s = 0.f;
+#pragma unroll
+  for (int t = 0; t < n; ++t) s += v[t] - k;
+  s += __shfl_xor_sync(0xffffffffu, s, 1);
+  s += __shfl_xor_sync(0xffffffffu, s, 2);
+  mu = k + s * (1.0f / (4 * n));
+  float q = 0.f;
+#pragma unroll
+  for (int t = 0; t < n; ++t) {
+    const float d = v[t] - mu;
+    q = fmaf(d, d, q);
+  }
+  q += __shfl_xor_sync(0xffffffffu, q, 1);
+  q += __shfl_xor_sync(0xffffffffu, q, 2);
+  rstd = rsqrtf(q * (1.0f / (4 * n)) + eps);
+}
+
 struct StepEpilogue {  // fused forecast-step epilogue of a narrow-output row MLP (see TcParams::ep_*)
   const float* prev;
   const float* boundary;

@@ -191,17 +191,8 @@ __device__ __forceinline__ void fz_layernorm(float (*v)[16], const float* gamma,
   const int cq = 2 * (threadIdx.x & 3);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    float sm = 0.f, sq = 0.f;
-#pragma unroll
-    for (int t = 0; t < 16; ++t) {
-      sm += v[i][t];
-      sq = fmaf(v[i][t], v[i][t], sq);
-    }
-    sm += __shfl_xor_sync(0xffffffffu, sm, 1);
-    sq += __shfl_xor_sync(0xffffffffu, sq, 1);
-    sm += __shfl_xor_sync(0xffffffffu, sm, 2);
-    sq += __shfl_xor_sync(0xffffffffu, sq, 2);
-    const float mu = sm * (1.0f / 64), rstd = rsqrtf(fmaxf(sq * (1.0f / 64) - mu * mu, 0.f) + eps);
+    float mu, rstd;
+    quad_row_stats<16>(v[i], eps, mu, rstd);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
 #pragma unroll

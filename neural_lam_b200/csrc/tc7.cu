@@ -176,20 +176,7 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         v[2 * j + 1] = acc[4 * j + 2 * i + 1] + sprm[8 * j + cq + 1];
       }
       float mu = 0.f, rstd = 1.f;
-      if (p.gamma) {  // LayerNorm statistics of the row: this thread's N / 4 columns, then the 4 threads of the quad
-        float sm = 0.f, sq = 0.f;
-#pragma unroll
-        for (int j = 0; j < N / 4; ++j) {
-          sm += v[j];
-          sq = fmaf(v[j], v[j], sq);
-        }
-        sm += __shfl_xor_sync(0xffffffffu, sm, 1);
-        sq += __shfl_xor_sync(0xffffffffu, sq, 1);
-        sm += __shfl_xor_sync(0xffffffffu, sm, 2);
-        sq += __shfl_xor_sync(0xffffffffu, sq, 2);
-        mu = sm * (1.0f / N);
-        rstd = rsqrtf(fmaxf(sq * (1.0f / N) - mu * mu, 0.f) + p.eps);
-      }
+      if (p.gamma) quad_row_stats<N / 4>(v, p.eps, mu, rstd);  // LayerNorm statistics of the row (all 4 quad lanes)
       if (!valid) continue;
       for (int a = 0; a < 2; ++a)
         if (p.add[a])
